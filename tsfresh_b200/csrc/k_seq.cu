@@ -7,9 +7,13 @@
 // open-addressing key table per Lempel-Ziv parameter, uint16 symbols, float xs[npad] (17.8 KB per warp at 256 samples,
 // run from the global working region); compact layout k_seq_small (series <= 256, alphabets <= 127) = packed 16-bit
 // histogram counters, 16-bit keys in 256-slot tables, byte symbols (6.5 KB per warp, shared memory, 32 warps per SM).
-// k_peaks (number_cwt_peaks): row0[npad], tmp[npad] (cwt rows, float64), noise[npad], hw[TSFX_MAXW_PTS] (wavelet taps),
-// float32 copies of the wider rows, a zero-padded float64 copy of the series in the working region; the ridge-line
-// tables (5 int16 + 3 int32 per line), the column map and the local-maximum bit masks in shared memory.
+// number_cwt_peaks: both kernels read the Ricker taps from a per-context table (launch_fill_ricker).
+// k_peaks_small (series <= 256 samples, register-blocked CWT): row0 (float64), float32 copies of the wider rows, the maxima bits
+// and a skewed float32 copy of the series that the packed ridge-line records and int16 column map reuse after the CWT
+// (8.3 KB per warp at 256 samples and n = 5, all in shared memory, 24 warps per SM).  k_peaks (longer series):
+// row0[npad], tmp[npad] (cwt rows, float64), noise[npad], float32 copies of the wider rows, a zero-padded float64 copy
+// of the series in the working region; the ridge-line tables (5 int16 + 3 int32 per line), the column map and the
+// local-maximum bit masks in shared memory.
 #include <algorithm>
 
 #include "tsfx_common.cuh"
@@ -26,7 +30,7 @@ struct SeqLayout {
                                                      // tables (ridge lines, column map, maxima bits) stay in shared memory
     int hist_cap;                                    // permutation-histogram bins the `codes` area can hold
     int npad, npow2, nwords, lz_lanes, cwt_n, lz_hash, lz_stride, nxd;
-    int off_rowsf, off_noise, off_hw, off_codes, off_trie, off_sym, off_bits, off_lines, off_map, off_xs, off_xd;   // byte offsets
+    int off_rowsf, off_noise, off_codes, off_trie, off_sym, off_bits, off_lines, off_map, off_xs, off_xd;   // byte offsets
 };
 
 // ---------------------------------------------------------------------------- Lempel-Ziv
@@ -64,11 +68,31 @@ __device__ __forceinline__ void warp_bitonic_sort_u32(unsigned* s, int m, int la
 }
 
 // ---------------------------------------------------------------------------- find_peaks_cwt pieces
-// cwt row of width w: dst[i] = convolve(x, ricker(npts, w), mode="same")[i] = sum_u h[u] x[i + c0 - u], c0 = (npts-1)/2.
-// xd is the series as float64 with TSFX_MAXW_PTS zeros in front and zeros up to a whole 256-sample chunk (+ the
-// same margin) behind, so no tap needs a bounds test.  Each lane forms 8 outputs (i = lane + 32 m) at once: one
-// broadcast load of the tap serves all of them, i.e. ~2.4 instructions per output tap instead of ~5.5.
-__device__ __forceinline__ void cwt_row(const double* xd, int n, const double* hw, int npts, double* dst, int lane) {
+// _ricker(points, a) (:1307-1316) depends on tap v only through vec = v - (points - 1) / 2, and on vec only through
+// vec^2, so one table row per width holds every tap of every points <= 10 w <= TSFX_RICKER_K: entry |2 vec|.  Filled
+// once per context on the device with scipy's expression (a host fill could round exp differently).
+__global__ void k_fill_ricker(double* tab) {
+    const int w = blockIdx.x + 1, k = threadIdx.x;
+    const double a = (double)w;
+    const double A = 2.0 / (sqrt(3.0 * a) * pow(3.14159265358979323846, 0.25));
+    const double wsq = a * a;
+    const double vec = 0.5 * (double)k;          // exact, as v - (points - 1) / 2 is
+    const double xsq = vec * vec;
+    const double mod = 1.0 - xsq / wsq;
+    const double gauss = exp(-xsq / (2.0 * wsq));
+    tab[(size_t)(w - 1) * TSFX_RICKER_K + k] = A * mod * gauss;
+}
+cudaError_t launch_fill_ricker(double* tab, cudaStream_t st) {
+    k_fill_ricker<<<TSFX_RICKER_W, TSFX_RICKER_K, 0, st>>>(tab);
+    return cudaGetLastError();
+}
+
+// k_peaks: cwt row of width w, dst[i] = sum_u h[u] x[i + c0 - u] as below, lane-interleaved (i = lane + 32 m).  xd is
+// the series as float64 with TSFX_MAXW_PTS zeros in front and zeros up to a whole 256-sample chunk (+ the same margin)
+// behind, so no tap needs a bounds test.  One broadcast load of the tap serves 8 outputs.  (From the global working
+// region the register-blocked form below measured slower: PEAKS 277 against 265 ms at 1 M x 1024 on an H100 SXM
+// with a 400 W power limit.)
+__device__ __forceinline__ void cwt_row(const double* xd, int n, const double* __restrict__ taps, int npts, double* dst, int lane) {
     const int c0 = (npts - 1) / 2;
     for (int i0 = 0; i0 < n; i0 += 256) {
         double acc[8];
@@ -76,7 +100,7 @@ __device__ __forceinline__ void cwt_row(const double* xd, int n, const double* h
         for (int m = 0; m < 8; ++m) acc[m] = 0.0;
         const double* xb = xd + TSFX_MAXW_PTS + i0 + lane + c0;
         for (int u = 0; u < npts; ++u) {
-            const double h = hw[u];
+            const double h = __ldg(taps + abs(2 * u - (npts - 1)));
 #pragma unroll
             for (int m = 0; m < 8; ++m) acc[m] = fma(xb[32 * m - u], h, acc[m]);
         }
@@ -88,19 +112,34 @@ __device__ __forceinline__ void cwt_row(const double* xd, int n, const double* h
     }
 }
 
-__device__ __forceinline__ void ricker_fill(double* hw, int npts, int w, int lane) {
-    // _ricker(points, a) (:1307-1316)
-    const double a = (double)w;
-    const double A = 2.0 / (sqrt(3.0 * a) * pow(3.14159265358979323846, 0.25));
-    const double wsq = a * a;
-    for (int v = lane; v < npts; v += 32) {
-        double vec = (double)v - ((double)npts - 1.0) / 2.0;
-        double xsq = vec * vec;
-        double mod = 1.0 - xsq / wsq;
-        double gauss = exp(-xsq / (2.0 * wsq));
-        hw[v] = A * mod * gauss;
+// k_peaks_small: CWT row of width w, register-blocked: the lane forms the 8 consecutive outputs i0 .. i0+7 of
+//   convolve(x, ricker(npts, w), mode="same")[i] = sum_u h[u] x[i + c0 - u],  c0 = (npts - 1) / 2,
+// each one fma-accumulated over u = 0 .. npts-1 from 0.0.  The 8 outputs' inputs slide down by one sample per tap, so a
+// window of 8 samples in registers costs one load per tap (and one tap load per 8 fma).  x(t) is sample t as float64,
+// zero outside 0 .. n-1; it is called for t = i0 + c0 - (npts - 1) .. i0 + 7 + c0.  taps = the width's table row.
+template <typename X>
+__device__ __forceinline__ void cwt_run8(X x, int i0, int npts, const double* __restrict__ taps, double (&acc)[8]) {
+    const int c0 = (npts - 1) / 2, base = i0 + c0;
+    double win[8];
+#pragma unroll
+    for (int m = 0; m < 8; ++m) acc[m] = 0.0;
+#pragma unroll
+    for (int m = 1; m < 8; ++m) win[m - 1] = x(base + m);      // moved into place by the first tap
+    win[7] = 0.0;
+    auto tap = [&](int u) {
+#pragma unroll
+        for (int m = 7; m > 0; --m) win[m] = win[m - 1];
+        win[0] = x(base - u);                                   // win[m] = x(i0 + m + c0 - u)
+        const double h = __ldg(taps + abs(2 * u - (npts - 1)));
+#pragma unroll
+        for (int m = 0; m < 8; ++m) acc[m] = fma(win[m], h, acc[m]);
+    };
+    int u = 0;
+    for (; u + 8 <= npts; u += 8) {
+#pragma unroll
+        for (int q = 0; q < 8; ++q) tap(u + q);
     }
-    __syncwarp();
+    for (; u < npts; ++u) tap(u);
 }
 
 // scipy.stats.scoreatpercentile(win[0..wlen), 10): the order statistics i = floor(0.1 (wlen-1)) and i+1 are
@@ -382,7 +421,6 @@ __global__ void __launch_bounds__(WPC * 32) k_peaks(SeqArgs A, SeqLayout Y) {
     double* tmp = row0 + Y.npad;                                           // npad : the row being formed
     double* noise = reinterpret_cast<double*>(base + Y.off_noise);         // npad : memoised noise floor (NaN = not yet)
     float* rowsf = reinterpret_cast<float*>(base + Y.off_rowsf);           // (cwt_n - 1) x npad : wider rows, float32 copies
-    double* hw = reinterpret_cast<double*>(base + Y.off_hw);
     // ridge-line bookkeeping is a chain of dependent small-table lookups: from the global region every one of them is
     // an L2 round trip (the hottest stalls of the kernel), so these tables get their own shared-memory slice
     unsigned char* hot = (GS && Y.hot_bytes > 0) ? smem_raw + (size_t)warp * Y.hot_bytes : nullptr;
@@ -412,9 +450,8 @@ __global__ void __launch_bounds__(WPC * 32) k_peaks(SeqArgs A, SeqLayout Y) {
                     // all rows 1..cwt_n once (kept in shared memory) + local-maximum bit masks per row
                     for (int w = 1; w <= Y.cwt_n; ++w) {
                         const int npts = min(10 * w, n);
-                        ricker_fill(hw, npts, w, lane);
                         double* dst = (w == 1) ? row0 : tmp;
-                        cwt_row(xd, n, hw, npts, dst, lane);
+                        cwt_row(xd, n, A.ricker + (size_t)(w - 1) * TSFX_RICKER_K, npts, dst, lane);
                         __syncwarp();
                         unsigned* bits = maxbits + (size_t)(w - 1) * Y.nwords;
                         for (int b0 = 0; b0 < n; b0 += 32) {
@@ -563,6 +600,208 @@ __global__ void __launch_bounds__(WPC * 32) k_peaks(SeqArgs A, SeqLayout Y) {
     }
 }
 
+// ---------------------------------------------------------------------------- k_peaks_small: series <= 256 samples
+// One register-blocked pass per CWT row (32 lanes x 8 outputs), everything in shared memory:
+//   row0     float64[npad]            width-1 row (noise floor and the SNR of lines ending in row 0)
+//   rowsf    float32[(cwt_n-1) npad]  wider rows, read only for the SNR test (float32, as k_peaks)
+//   bits     uint32[cwt_n][8]         local-maximum masks, one byte per lane
+//   union    the series as float32, skewed (xz_at) with PK_XZ_FRONT zeros in front and zeros behind, while the rows
+//            are formed; then the ridge lines (one packed uint32 per line, LCAP of them) and the int16 column map
+// The noise floor is recomputed per accepted-length line instead of memoised: windows are <= 13 samples here.
+#define PK_SMALL_LEN 256
+#define PK_XZ_FRONT 80                  // widest tap reach behind an output: 160 taps, c0 = 79
+#define PK_XZ_LOGICAL (PK_XZ_FRONT + PK_SMALL_LEN + 79)       // t = -80 .. 334
+#define PK_XZ_FLOATS 428                // xz_at(PK_XZ_LOGICAL - 1) + 1, rounded up to 16 bytes
+// A lane reads samples 8 apart; one unused float per 32 spreads a warp's 32 reads over distinct banks
+__device__ __forceinline__ int xz_at(int p) { return p + (p >> 5); }
+
+// line record: last column | first column of the latest row << 8 | latest row << 16 | gap << 20 | length << 24.  The
+// length saturates at 255: it is only compared with min_length = ceil(n / 4) <= 4.
+#define LN_REC(last, col, row, len) ((unsigned)(last) | ((unsigned)(col) << 8) | ((unsigned)(row) << 16) | ((unsigned)(len) << 24))
+#define LN_LAST(r) ((int)((r) & 0xffu))
+#define LN_COL(r) ((int)(((r) >> 8) & 0xffu))
+#define LN_ROW(r) ((int)(((r) >> 16) & 0xfu))
+#define LN_GAP(r) ((int)(((r) >> 20) & 0xfu))
+#define LN_LEN(r) ((int)((r) >> 24))
+
+template <int WPC>
+__global__ void __launch_bounds__(WPC * 32, 24 / WPC) k_peaks_small(SeqArgs A, SeqLayout Y) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned char* base = smem_raw + (size_t)warp * A.bytes_per_warp;
+    double* row0 = reinterpret_cast<double*>(base);
+    float* rowsf = reinterpret_cast<float*>(base + Y.off_rowsf);
+    unsigned* maxbits = reinterpret_cast<unsigned*>(base + Y.off_bits);
+    float* xz = reinterpret_cast<float*>(base + Y.off_xs);                 // while the rows are formed
+    unsigned* lines = reinterpret_cast<unsigned*>(base + Y.off_lines);     // afterwards, over the same bytes
+    short* colmap = reinterpret_cast<short*>(base + Y.off_map);
+    const int64_t warps_total = (int64_t)gridDim.x * WPC;
+    const int LCAP = Y.npad + Y.npad / 2 + 32;   // alive (<= maxima of the two previous rows <= n) + new in this row (<= n/2)
+    const unsigned lt = (1u << lane) - 1u;
+    const int NONE = 0x7fff;
+    auto xat = [&](int t) { return (double)xz[xz_at(t + PK_XZ_FRONT)]; };
+
+    for (int64_t s = (int64_t)blockIdx.x * WPC + warp; s < A.R.n_series; s += warps_total) {
+        int64_t b;
+        int n;
+        if (A.R.begin) { b = A.R.begin[s]; n = A.R.len[s]; } else { b = s * (int64_t)A.R.dense_len; n = A.R.dense_len; }
+        // all rows 1..cwt_n first (every descriptor of the group is number_cwt_peaks)
+        const float* src = A.R.values + b;
+        for (int p = lane; p < PK_XZ_LOGICAL; p += 32) {
+            const int t = p - PK_XZ_FRONT;
+            xz[xz_at(p)] = (t >= 0 && t < n) ? __ldg(src + t) : 0.f;
+        }
+        __syncwarp();
+        const int i0 = 8 * lane;
+        for (int w = 1; w <= Y.cwt_n; ++w) {
+            double v[8];
+            cwt_run8(xat, i0, min(10 * w, n), A.ricker + (size_t)(w - 1) * TSFX_RICKER_K, v);
+            // strict local maxima, the ends excluded (scipy compares them with themselves)
+            const double vl = __shfl_up_sync(FULL, v[7], 1), vr = __shfl_down_sync(FULL, v[0], 1);
+            unsigned mb = 0;
+#pragma unroll
+            for (int m = 0; m < 8; ++m) {
+                const double l = m > 0 ? v[m - 1] : vl, r = m < 7 ? v[m + 1] : vr;
+                const int i = i0 + m;
+                if (i >= 1 && i <= n - 2 && v[m] > l && v[m] > r) mb |= 1u << m;
+            }
+            reinterpret_cast<unsigned char*>(maxbits + (w - 1) * 8)[lane] = (unsigned char)mb;
+            if (w == 1) {
+                if (i0 + 8 <= n) {
+#pragma unroll
+                    for (int m = 0; m < 8; m += 2) *reinterpret_cast<double2*>(row0 + i0 + m) = make_double2(v[m], v[m + 1]);
+                } else {
+#pragma unroll
+                    for (int m = 0; m < 8; ++m) if (i0 + m < n) row0[i0 + m] = v[m];
+                }
+            } else {
+                float* rf = rowsf + (size_t)(w - 2) * Y.npad;
+                if (i0 + 8 <= n) {
+                    *reinterpret_cast<float4*>(rf + i0) = make_float4((float)v[0], (float)v[1], (float)v[2], (float)v[3]);
+                    *reinterpret_cast<float4*>(rf + i0 + 4) = make_float4((float)v[4], (float)v[5], (float)v[6], (float)v[7]);
+                } else {
+#pragma unroll
+                    for (int m = 0; m < 8; ++m) if (i0 + m < n) rf[i0 + m] = (float)v[m];
+                }
+            }
+        }
+        __syncwarp();                   // xz is dead from here on: its bytes hold the lines
+        double* orow = A.out + (size_t)s * A.ncols;
+        int j = 0;
+        while (j < A.nd) {
+            const Desc d0 = A.descs[j];
+            if (d0.calc == TSFX_NUMBER_CWT_PEAKS) {
+                const int nrows = d0.i0;
+                // ---- ridge lines (scipy _identify_ridge_lines + _filter_ridge_lines), as k_peaks ----
+                const int min_length = (nrows + 3) / 4;                       // ceil(nrows / 4)
+                int result = 0, nl = 0, start = -1;
+                for (int r = nrows - 1; r >= 0 && start < 0; --r) {             // largest row with any maximum
+                    const unsigned* bits = maxbits + r * 8;
+                    unsigned any = 0;
+                    for (int wd = lane; wd * 32 < n; wd += 32) any |= bits[wd];
+                    if (__any_sync(FULL, any != 0)) start = r;
+                }
+                if (start >= 0) {
+                    const unsigned* bits = maxbits + start * 8;
+                    for (int b0 = 0; b0 < n; b0 += 32) {
+                        const unsigned word = bits[b0 >> 5];
+                        const int idx = nl + __popc(word & lt);
+                        if (((word >> lane) & 1u) && idx < LCAP) lines[idx] = LN_REC(b0 + lane, b0 + lane, start, 1);
+                        nl = min(nl + __popc(word), LCAP);
+                    }
+                }
+                __syncwarp();
+                const int window = (n + 19) / 20, hf = window / 2, odd = window & 1;
+                auto accept = [&](unsigned rec) -> bool {
+                    if (LN_LEN(rec) < min_length) return false;
+                    const int rr = LN_ROW(rec), cc = LN_COL(rec);
+                    const int ws = max(cc - hf, 0), we = min(cc + hf + odd, n);
+                    const double nz = percentile10(row0 + ws, we - ws);
+                    const double val = (rr == 0) ? row0[cc] : (double)rowsf[(size_t)(rr - 1) * Y.npad + cc];
+                    const double snr = fabs(val / nz);
+                    return !(snr < 1.0);
+                };
+                for (int r = start - 1; r >= 0; --r) {
+                    const unsigned* bits = maxbits + r * 8;
+                    const int maxd = (r + 1) / 4;                  // floor(widths[r] / 4); distances are integers
+                    for (int c = lane; c < n; c += 32) colmap[c] = (short)NONE;
+                    for (int li = lane; li < nl; li += 32) lines[li] += 1u << 20;      // gap + 1
+                    __syncwarp();
+                    // snapshot: column -> first line (list order) whose last column is that column.  Chunks from the
+                    // back, the lowest lane of equal columns stores: the smallest line index is written last
+                    for (int b0 = (nl - 1) & ~31; b0 >= 0; b0 -= 32) {
+                        const int li = b0 + lane;
+                        const int key = li < nl ? LN_LAST(lines[li]) : -1;
+                        const unsigned grp = __match_any_sync(FULL, key);
+                        if (key >= 0 && (grp & lt) == 0) colmap[key] = (short)li;
+                        __syncwarp();
+                    }
+                    const int nl_snapshot = nl;
+                    for (int b0 = 0; b0 < n; b0 += 32) {
+                        const unsigned word = bits[b0 >> 5];
+                        const bool mine = (word >> lane) & 1u;
+                        const int c = b0 + lane;
+                        int best = -1;
+                        if (mine && nl_snapshot > 0) {
+                            // np.argmin(|c - prev|): smallest distance, first in list order on ties; attach only
+                            // when that distance is <= max_distances[row]
+                            for (int dd = 0; dd <= maxd && best < 0; ++dd) {
+                                const int a = (c - dd >= 0) ? colmap[c - dd] : NONE;
+                                const int bb = (dd > 0 && c + dd < n) ? colmap[c + dd] : NONE;
+                                const int m = min(a, bb);
+                                if (m != NONE) best = m;
+                            }
+                        }
+                        // columns of this chunk that attach to one line: the lowest lane updates the record (columns
+                        // ascend, so the first attachment of the row sets the row's first column, the last one `last`)
+                        const unsigned grp = __match_any_sync(FULL, best);
+                        if (best >= 0 && (grp & lt) == 0) {
+                            const unsigned rec = lines[best];
+                            const int col = LN_GAP(rec) != 0 ? c : LN_COL(rec);       // gap 0: attached earlier in this row
+                            lines[best] = LN_REC(b0 + 31 - __clz(grp), col, r, min(LN_LEN(rec) + __popc(grp), 255));
+                        }
+                        const unsigned newm = __ballot_sync(FULL, mine && best < 0);
+                        if (mine && best < 0) {
+                            const int idx = nl + __popc(newm & lt);
+                            if (idx < LCAP) lines[idx] = LN_REC(c, c, r, 1);
+                        }
+                        nl = min(nl + __popc(newm), LCAP);
+                        __syncwarp();
+                    }
+                    // retire lines whose gap exceeds gap_thresh = ceil(widths[0]) = 1; survivors keep their order
+                    int keep = 0;
+                    for (int b0 = 0; b0 < nl; b0 += 32) {
+                        const int li = b0 + lane;
+                        const bool valid = li < nl;
+                        const unsigned rec = valid ? lines[li] : 0u;
+                        const bool retire = valid && LN_GAP(rec) > 1;
+                        const bool ok = retire && accept(rec);
+                        result += __popc(__ballot_sync(FULL, ok));
+                        const unsigned keepm = __ballot_sync(FULL, valid && !retire);
+                        __syncwarp();
+                        if (valid && !retire) lines[keep + __popc(keepm & lt)] = rec;
+                        keep += __popc(keepm);
+                        __syncwarp();
+                    }
+                    nl = keep;
+                }
+                for (int b0 = 0; b0 < nl; b0 += 32) {
+                    const int li = b0 + lane;
+                    const bool ok = li < nl && accept(lines[li]);
+                    result += __popc(__ballot_sync(FULL, ok));
+                }
+                if (lane == 0) orow[d0.col] = (double)result;
+                __syncwarp();
+                ++j;
+            } else {
+                if (lane == 0) orow[d0.col] = dnan();
+                ++j;
+            }
+        }
+        __syncwarp();
+    }
+}
+
 // lempel_ziv_complexity + permutation_entropy
 cudaError_t launch_seq(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_count) {
     SeqArgs A = A0;
@@ -629,14 +868,40 @@ cudaError_t launch_peaks(const SeqArgs& A0, int max_len, cudaStream_t st, int sm
     SeqArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     if (max_len > 32000) return cudaErrorInvalidConfiguration;      // int16 line tables
+    if (!A.ricker) return cudaErrorInvalidValue;
     SeqLayout Y = {};
     Y.npad = A.npad;
-    Y.nwords = (A.npad + 31) / 32 + 1;
     Y.cwt_n = (A.nscr >> 8) & 0xff;
+    if (Y.cwt_n < 1 || Y.cwt_n > TSFX_RICKER_W) return cudaErrorInvalidValue;
+    if (max_len <= PK_SMALL_LEN) {
+        // k_peaks_small while its footprint keeps at least 16 warps per SM resident (at 256 samples: n <= 10)
+        const size_t lcap = (size_t)A.npad + A.npad / 2 + 32;
+        size_t o = (size_t)A.npad * 8;                                       // row0
+        Y.off_rowsf = (int)o; o += (size_t)(Y.cwt_n - 1) * A.npad * 4;
+        Y.nwords = PK_SMALL_LEN / 32;
+        Y.off_bits = (int)o;  o += (size_t)Y.cwt_n * Y.nwords * 4;
+        o = (o + 15) & ~(size_t)15;
+        Y.off_xs = Y.off_lines = (int)o;
+        Y.off_map = (int)(o + lcap * 4);
+        o += std::max((size_t)PK_XZ_FLOATS * 4, lcap * 4 + (size_t)A.npad * 2);
+        const size_t per = (o + 15) & ~(size_t)15;
+        if (4 * (4 * per + 1024) <= 228 * 1024) {
+            A.bytes_per_warp = (int)per;
+            A.gscratch = nullptr;
+            const size_t smem = per * 4;
+            const int64_t ctas = (A.R.n_series + 3) / 4;
+            const int64_t cap = (int64_t)sm_count * grid_waves(4096);
+            const int grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
+            cudaError_t e = cudaFuncSetAttribute(k_peaks_small<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+            if (e != cudaSuccess) return e;
+            k_peaks_small<4><<<grid, 4 * 32, smem, st>>>(A, Y);
+            return cudaGetLastError();
+        }
+    }
+    Y.nwords = (A.npad + 31) / 32 + 1;
     size_t off = 0;
     off += (size_t)2 * A.npad * 8;                          // row0 + tmp (float64)
     Y.off_noise = (int)off; off += (size_t)A.npad * 8;
-    Y.off_hw = (int)off;    off += (size_t)TSFX_MAXW_PTS * 8;
     Y.off_bits = (int)off;  off += (size_t)Y.cwt_n * Y.nwords * 4;
     off = (off + 3) & ~(size_t)3;
     Y.off_rowsf = (int)off; off += (size_t)std::max(Y.cwt_n - 1, 0) * A.npad * 4;

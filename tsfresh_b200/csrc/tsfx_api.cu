@@ -233,6 +233,7 @@ struct tsfx_ctx {
     double* d_dec = nullptr;
     double2* d_tw = nullptr;
     int tw_n = 0;
+    double* d_ricker = nullptr;           // number_cwt_peaks tap table (TSFX_RICKER_W x TSFX_RICKER_K), filled on first use
     cudaEvent_t ev[G_EVENTS][2];
     bool ev_used[G_EVENTS];
     float ms[G_EVENTS];
@@ -407,6 +408,7 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     if (ctx->ev_peer) cudaEventDestroy(ctx->ev_peer);
     if (ctx->d_dec) cudaFree(ctx->d_dec);
     if (ctx->d_tw) cudaFree(ctx->d_tw);
+    if (ctx->d_ricker) cudaFree(ctx->d_ricker);
     for (int g = 0; g < G_EVENTS; ++g) { if (ctx->ev[g][0]) cudaEventDestroy(ctx->ev[g][0]); if (ctx->ev[g][1]) cudaEventDestroy(ctx->ev[g][1]); }
     for (int i = 0; i < 3; ++i) { if (ctx->s_side[i]) cudaStreamDestroy(ctx->s_side[i]); if (ctx->ev_join[i]) cudaEventDestroy(ctx->ev_join[i]); }
     if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
@@ -579,6 +581,13 @@ static int ensure_twiddle(tsfx_ctx* ctx, int n_pow2) {
     return TSFX_OK;
 }
 
+static int ensure_ricker(tsfx_ctx* ctx) {
+    if (ctx->d_ricker) return TSFX_OK;
+    CK(cudaMalloc(&ctx->d_ricker, (size_t)TSFX_RICKER_W * TSFX_RICKER_K * sizeof(double)));
+    CK(launch_fill_ricker(ctx->d_ricker, ctx->stream));
+    return TSFX_OK;
+}
+
 // row timestamps handed over with tsfx_set_row_times for a call whose `values` array has `rows` rows (consumed)
 static int take_times(tsfx_ctx* ctx, const tsfx_plan* P, int64_t rows, const int64_t** out) {
     *out = nullptr;
@@ -626,6 +635,10 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         if (p2 > max_len) p2 >>= 1;            // largest power of two <= max_len
         p2 = std::max(p2, 256);
         int rc = ensure_twiddle(ctx, p2);
+        if (rc) return rc;
+    }
+    if (!P->host[G_PEAKS].empty()) {         // Ricker taps (filled once, on the main stream, before any fork)
+        int rc = ensure_ricker(ctx);
         if (rc) return rc;
     }
     // kernel groups are independent (own staging matrix): optionally spread them over side streams
@@ -740,6 +753,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                 SeqArgs A;
                 A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
                 A.nscr = (P->max_cwt_peaks_n << 8);
+                A.ricker = ctx->d_ricker;
                 e = launch_peaks(A, max_len, gs, ctx->sm_count);
                 break;
             }

@@ -199,9 +199,16 @@ struct SeqArgs {
     double* out;
     int ncols;
     int npad, nscr, bytes_per_warp;
+    const double* ricker = nullptr;    // PEAKS: device Ricker tap table (launch_fill_ricker)
 };
 cudaError_t launch_seq(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count);
 cudaError_t launch_peaks(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count);
+
+// Ricker tap table of number_cwt_peaks: widths 1..TSFX_RICKER_W, entry (w - 1) * TSFX_RICKER_K + |2 v - (points - 1)|
+// is tap v of ricker(points, w) for every points <= 10 w (filled once per context, on the device)
+#define TSFX_RICKER_W 16
+#define TSFX_RICKER_K 160
+cudaError_t launch_fill_ricker(double* tab, cudaStream_t st);
 
 // plain fill of a column set with NaN is done by BASIC (TSFX_CONST_NAN)
 
