@@ -319,6 +319,13 @@ int tsfx_select_regression(tsfx_ctx* ctx, const double* X, int64_t n_rows, int32
 int tsfx_get_timings(tsfx_ctx* ctx, float* ms_out, const char** names_out, int32_t cap);
 /* Number of kernels the last extract call launched. */
 int tsfx_last_launch_count(const tsfx_ctx* ctx);
+/* Which kernel variant each kernel group of the last extract call ran, e.g. "entropy/rank-g4", "basic/w12/shared",
+ * "spectral/w4/global", "peaks/general/hybrid", "moments/dense" (entry points that work in row blocks: the last
+ * block).  names_out[i] points at a static string.  Returns the number of groups written (<= cap). */
+int tsfx_last_kernels(const tsfx_ctx* ctx, const char** names_out, int32_t cap);
+/* Every variant name tsfx_last_kernels can report, including those only A/B tuning variables select.  Returns the
+ * number of names; writes at most cap of them to names_out (may be NULL). */
+int tsfx_kernel_variants(const char** names_out, int32_t cap);
 
 #ifdef __cplusplus
 }

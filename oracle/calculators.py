@@ -625,8 +625,29 @@ def sample_entropy(x):  # :1701-1754
         return -np.log(A / B)
 
 
-@simple
-def approximate_entropy(x, m, r):  # :1759-1805
+APEN_BLOCK_ELEMENTS = 1 << 22      # float64 elements of one block of the pairwise distance matrix (32 MB)
+
+
+def _apen_counts(w, r, block_cols):
+    """counts[j] = #{i : max_k |w[i, k] - w[j, k]| <= r}, evaluated on [n x block_cols] slices of the distance matrix
+    (None: the whole [n x n x mm] array at once, as the reference does).  The maximum of the absolute differences is
+    exact in any order, so every block size gives the same integer counts."""
+    n = len(w)
+    if block_cols is None:
+        return np.sum(np.max(np.abs(w[:, None] - w[None, :]), axis=2) <= r, axis=0)
+    counts = np.empty(n, dtype=np.int64)
+    for j0 in range(0, n, block_cols):
+        j1 = min(n, j0 + block_cols)
+        d = np.abs(w[:, 0, None] - w[None, j0:j1, 0])
+        for k in range(1, w.shape[1]):
+            np.maximum(d, np.abs(w[:, k, None] - w[None, j0:j1, k]), out=d)
+        counts[j0:j1] = np.sum(d <= r, axis=0)
+    return counts
+
+
+def approximate_entropy_blocked(x, m, r, block_cols=0):
+    """approximate_entropy with the match counts taken over column blocks of the distance matrix; block_cols=0 sizes
+    the blocks to APEN_BLOCK_ELEMENTS, None forms the full N x N x m array (the reference's memory footprint)."""
     N = x.size
     r = r * np.std(x)
     if r < 0:
@@ -636,10 +657,16 @@ def approximate_entropy(x, m, r):  # :1759-1805
 
     def phi(mm):
         w = np.array([x[i:i + mm] for i in range(N - mm + 1)])
-        C = np.sum(np.max(np.abs(w[:, None] - w[None, :]), axis=2) <= r, axis=0) / (N - mm + 1)
+        cols = block_cols if block_cols is None or block_cols > 0 else max(1, APEN_BLOCK_ELEMENTS // len(w))
+        C = _apen_counts(w, r, cols) / (N - mm + 1)
         return np.sum(np.log(C)) / (N - mm + 1.0)
 
     return np.abs(phi(m) - phi(m + 1))
+
+
+@simple
+def approximate_entropy(x, m, r):  # :1759-1805
+    return approximate_entropy_blocked(x, m, r)
 
 
 @simple

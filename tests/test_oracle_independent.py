@@ -121,3 +121,25 @@ def test_cwt_restatement_against_exact_integration_of_the_mexican_hat(scale, kin
         # kernel that a rough signal does not average out (up to ~18 % of the largest coefficient at scale 20); the two
         # transforms are still the same transform
         assert np.corrcoef(exact, got)[0, 1] > 0.98
+
+
+# approximate_entropy: the oracle counts template matches over column blocks of the distance matrix, so that series of
+# 21 000 samples need 32 MB instead of an N x N x m array of 10 GB.  The counts are integers and the maximum of the
+# absolute differences is exact in any order, so the blocked form must equal the whole-array form bit for bit.
+def _apen_inputs():
+    rng = np.random.default_rng(11)
+    out = [rng.standard_normal(n) for n in (1, 2, 3, 4, 5, 8, 33, 100, 257, 600)]
+    out += [rng.standard_normal(600).cumsum(), np.round(rng.standard_normal(600) * 2) / 2,      # walk, many ties
+            np.zeros(50), np.full(300, 3.25), np.array([-1.0, 1.0] * 150), np.arange(200, dtype=np.float64)]
+    return [np.asarray(x, dtype=np.float32).astype(np.float64) for x in out]
+
+
+@pytest.mark.parametrize("m,r", [(2, 0.1), (2, 0.3), (2, 0.5), (2, 0.7), (2, 0.9), (3, 0.2)])
+def test_approximate_entropy_blocked_equals_whole_array(m, r):
+    from oracle import calculators
+    for x in _apen_inputs():
+        whole = calculators.approximate_entropy_blocked(x, m, r, block_cols=None)
+        for cols in (0, 1, 7, 64):
+            got = calculators.approximate_entropy_blocked(x, m, r, block_cols=cols)
+            assert got == whole or (np.isnan(got) and np.isnan(whole)), (len(x), cols, got, whole)
+        assert calculators.approximate_entropy(x, m, r) == whole or np.isnan(whole)

@@ -28,7 +28,7 @@ _lock = threading.Lock()
 EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync", "tsfx_version",
            "tsfx_plan_create", "tsfx_plan_destroy", "tsfx_extract_csr", "tsfx_extract_dense",
            "tsfx_extract_long", "tsfx_build_csr", "tsfx_roll_windows", "tsfx_get_timings",
-           "tsfx_last_launch_count", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
+           "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression"]
 
 
@@ -60,6 +60,8 @@ def load():
         lib.tsfx_roll_windows.restype = i64
         lib.tsfx_get_timings.argtypes = [vp, vp, vp, i32]
         lib.tsfx_last_launch_count.argtypes = [vp]
+        lib.tsfx_last_kernels.argtypes = [vp, vp, i32]
+        lib.tsfx_kernel_variants.argtypes = [vp, i32]
         lib.tsfx_impute.argtypes = [vp, vp, i64, i32, i32, vp, u32]
         lib.tsfx_extract_long_alloc.argtypes = [vp, vp, vp, vp, i32, vp, i64, ctypes.POINTER(vp), ctypes.POINTER(vp),
                                                 ctypes.POINTER(i64), u32]
@@ -81,6 +83,15 @@ def load():
 
 def device_count():
     return int(load().tsfx_device_count())
+
+
+def kernel_variants():
+    """Every kernel variant name Context.last_kernels can report."""
+    lib = load()
+    n = lib.tsfx_kernel_variants(None, 0)
+    names = (ctypes.c_char_p * n)()
+    lib.tsfx_kernel_variants(names, n)
+    return [names[i].decode() for i in range(n)]
 
 
 def _ptr(a):
@@ -136,6 +147,14 @@ class Context:
 
     def launch_count(self):
         return int(self.lib.tsfx_last_launch_count(self.h))
+
+    def last_kernels(self):
+        """The kernel variant every group of the last extract call ran (e.g. "basic/w12/shared"), in group order."""
+        names = (ctypes.c_char_p * 16)()
+        k = self.lib.tsfx_last_kernels(self.h, names, 16)
+        if k < 0:
+            self.check(k, "tsfx_last_kernels")
+        return [names[i].decode() for i in range(k)]
 
     def impute(self, matrix, mode=IMPUTE_RANGE, col_stats=None, all_medians=False):
         """tsfx_impute on a host matrix (C-contiguous float64 [rows x cols]), in place.  Returns the

@@ -893,7 +893,8 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
 bool basic_finisher_calc(int calc) { return basic_is_finisher(calc); }
 
 // ------------------------------------------------------------------------------------------ launcher
-cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("basic");
     BasicArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     A.nxc = ((max_len + 255) / 256) * 256 + ((A.lag_needed + 1) & ~1);      // centred copy + zero tail for the lag products
@@ -914,10 +915,10 @@ cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int 
     A.desc_bytes = (int)(((size_t)A.nd * sizeof(Desc) + 15) & ~(size_t)15);
     Geometry G;
     const size_t budget = (size_t)100 * 1024 > (size_t)A.desc_bytes + per ? (size_t)100 * 1024 - A.desc_bytes : per;
-    if (!plan_geometry(per, budget, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
+    // the CTA-wide descriptor table in front of the per-warp regions counts in the shared-versus-global choice
+    if (!plan_geometry(per, budget, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G, 227 * 1024, 0, A.desc_bytes))
+        return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    G.smem += A.desc_bytes;                       // CTA-wide descriptor table in front of the per-warp regions
-    if (G.smem > 227 * 1024) return cudaErrorInvalidConfiguration;
     {
         // Two CTAs of 12 warps per SM instead of three of 8 (TSFX_BASIC_WPC=8|12|24): all warps of a CTA walk the descriptor
         // list in lock step, so larger CTAs share more of the 250 KB instruction stream -- measured on H100 SXM (700 W) at
@@ -931,6 +932,7 @@ cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int 
                 const int64_t cap = (int64_t)sm_count * grid_waves(4096);
                 const int grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
                 cudaError_t e;
+                *variant = wide == 12 ? "basic/w12/shared" : "basic/w24/shared";
                 if (wide == 12) {
                     e = cudaFuncSetAttribute(k_basic<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
                     if (e != cudaSuccess) return e;
@@ -944,6 +946,7 @@ cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int 
             }
         }
     }
+    *variant = geom_variant(names, G);
     TSFX_DISPATCH(k_basic, G, st, A)
     return cudaGetLastError();
 }

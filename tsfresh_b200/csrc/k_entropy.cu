@@ -583,7 +583,9 @@ static cudaError_t launch_rank(const EntropyArgs& A, size_t smem, int ctas_per_s
     return cudaGetLastError();
 }
 
-cudaError_t launch_entropy(const EntropyArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_entropy(const EntropyArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("entropy/tiles");
+    static const char* const names_pairs[6] = TSFX_GEOM_NAMES("entropy/pairs");
     EntropyArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     A.xpad = ((A.npad + 2 + 31) / 32) * 32 + 32;          // NaN padding up to a whole 32-sample tile / 32-row block
@@ -602,9 +604,12 @@ cudaError_t launch_entropy(const EntropyArgs& A0, int max_len, cudaStream_t st, 
         const size_t s4 = lnk + (size_t)rank_layout(A.npad, 4, 1).bytes;
         const size_t s16 = lnk + (size_t)rank_layout(A.npad, 16, 1).bytes;
         const size_t sm_bytes = 227 * 1024;
-        if (s1 <= 75 * 1024) return launch_rank<1, 4>(A, s1, (int)std::min<size_t>(4, sm_bytes / (s1 + 1024)), st, sm_count);
-        if (s4 <= 55 * 1024) return launch_rank<4, 1>(A, s4, 4, st, sm_count);
-        if (s16 <= 226 * 1024) return launch_rank<16, 1>(A, s16, 1, st, sm_count);
+        if (s1 <= 75 * 1024) {
+            *variant = "entropy/rank-g1";
+            return launch_rank<1, 4>(A, s1, (int)std::min<size_t>(4, sm_bytes / (s1 + 1024)), st, sm_count);
+        }
+        if (s4 <= 55 * 1024) { *variant = "entropy/rank-g4"; return launch_rank<4, 1>(A, s4, 4, st, sm_count); }
+        if (s16 <= 226 * 1024) { *variant = "entropy/rank-g16"; return launch_rank<16, 1>(A, s16, 1, st, sm_count); }
     }
     size_t per = (size_t)A.xpad * 8 + (size_t)(A.npad + 4) * 8 + (size_t)A.npad * 4;
     per = (per + 15) & ~(size_t)15;
@@ -612,6 +617,7 @@ cudaError_t launch_entropy(const EntropyArgs& A0, int max_len, cudaStream_t st, 
     Geometry G;
     if (!plan_geometry(per, 64 * 1024, 4, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
+    *variant = geom_variant(A.bittile ? names : names_pairs, G);
     TSFX_DISPATCH(k_entropy, G, st, A)
     return cudaGetLastError();
 }

@@ -275,7 +275,8 @@ __global__ void __launch_bounds__(WPC * 32) k_la(LaArgs A, int pmax) {
     }
 }
 
-cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("la");
     LaArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     if (adf_maxlag(max_len) + 2 > 64) return cudaErrorInvalidConfiguration;     // autolag keeps one model per lane, two rounds
@@ -287,6 +288,7 @@ cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_cou
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
+    *variant = geom_variant(names, G);
     TSFX_DISPATCH(k_la, G, st, A, pmax)
     return cudaGetLastError();
 }

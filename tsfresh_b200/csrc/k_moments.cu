@@ -306,7 +306,7 @@ __global__ void __launch_bounds__(WPC * 32, 2) k_moments_dense(MomentsArgs A) {
     }
 }
 
-cudaError_t launch_moments(const MomentsArgs& A, cudaStream_t st, int sm_count) {
+cudaError_t launch_moments(const MomentsArgs& A, cudaStream_t st, int sm_count, const char** variant) {
     constexpr int SUB = 8, WPC = 8;
     const int64_t per_cta = (int64_t)WPC * (32 / SUB);
     int64_t ctas = (A.R.n_series + per_cta - 1) / per_cta;
@@ -319,9 +319,11 @@ cudaError_t launch_moments(const MomentsArgs& A, cudaStream_t st, int sm_count) 
         const int64_t cap2 = (int64_t)sm_count * 2 * grid_waves(1);          // persistent: two CTAs per SM, prefetching
         int64_t c2 = (A.R.n_series + per_cta - 1) / per_cta;
         if (c2 > cap2) c2 = cap2;
+        *variant = "moments/dense";
         k_moments_dense<SUB, WPC, 8><<<(int)c2, WPC * 32, 0, st>>>(A);
         return cudaGetLastError();
     }
+    *variant = "moments/general";
     k_moments<SUB, WPC, 8><<<(int)ctas, WPC * 32, 0, st>>>(A);
     return cudaGetLastError();
 }

@@ -803,7 +803,8 @@ __global__ void __launch_bounds__(WPC * 32, 24 / WPC) k_peaks_small(SeqArgs A, S
 }
 
 // lempel_ziv_complexity + permutation_entropy
-cudaError_t launch_seq(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_seq(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("seq/general");
     SeqArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     if (max_len > 21000) return cudaErrorInvalidConfiguration;      // LZ node ids are 15-bit slot indices
@@ -841,6 +842,7 @@ cudaError_t launch_seq(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_c
             const int64_t cap = (int64_t)sm_count * grid_waves(4096);
             G.grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
             A.gscratch = nullptr;
+            *variant = "seq/small";
             cudaError_t e = cudaFuncSetAttribute(k_seq_small<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G.smem);
             if (e != cudaSuccess) return e;
             k_seq_small<4, false><<<G.grid, 4 * 32, G.smem, st>>>(A, Y);
@@ -859,12 +861,16 @@ cudaError_t launch_seq(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_c
     Geometry G;
     if (!plan_geometry(per, 72 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G, 16 * 1024, 8)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
+    *variant = geom_variant(names, G);
     TSFX_DISPATCH(k_seq, G, st, A, Y)
     return cudaGetLastError();
 }
 
 // number_cwt_peaks
-cudaError_t launch_peaks(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_peaks(const SeqArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("peaks/general");
+    // global region with the hot tables in shared memory (only ever global, so its shared names are never reported)
+    static const char* const names_hybrid[6] = TSFX_GEOM_NAMES("peaks/general/hybrid");
     SeqArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     if (max_len > 32000) return cudaErrorInvalidConfiguration;      // int16 line tables
@@ -892,6 +898,7 @@ cudaError_t launch_peaks(const SeqArgs& A0, int max_len, cudaStream_t st, int sm
             const int64_t ctas = (A.R.n_series + 3) / 4;
             const int64_t cap = (int64_t)sm_count * grid_waves(4096);
             const int grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
+            *variant = "peaks/small";
             cudaError_t e = cudaFuncSetAttribute(k_peaks_small<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
             k_peaks_small<4><<<grid, 4 * 32, smem, st>>>(A, Y);
@@ -931,6 +938,7 @@ cudaError_t launch_peaks(const SeqArgs& A0, int max_len, cudaStream_t st, int sm
             G.smem = hot * G.wpc;
         }
     }
+    *variant = geom_variant(Y.hot_bytes ? names_hybrid : names, G);
     TSFX_DISPATCH(k_peaks, G, st, A, Y)
     return cudaGetLastError();
 }

@@ -403,7 +403,8 @@ bool sorted_finisher_calc(int calc) {
     }
 }
 
-cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, int sm_count) {
+cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+    static const char* const names[6] = TSFX_GEOM_NAMES("sorted");
     SortedArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     int p2 = 1;
@@ -425,12 +426,14 @@ cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, in
             const size_t smem = per * 12;
             const int64_t ctas = (A.R.n_series + 11) / 12;
             const int64_t cap = (int64_t)sm_count * grid_waves(4096);
+            *variant = "sorted/w12/shared";
             cudaError_t e = cudaFuncSetAttribute(k_sorted<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
             if (e != cudaSuccess) return e;
             k_sorted<12, false><<<(int)std::max<int64_t>(1, std::min(ctas, cap)), 12 * 32, smem, st>>>(A);
             return cudaGetLastError();
         }
     }
+    *variant = geom_variant(names, G);
     TSFX_DISPATCH(k_sorted, G, st, A)
     return cudaGetLastError();
 }

@@ -238,6 +238,8 @@ struct tsfx_ctx {
     bool ev_used[G_EVENTS];
     float ms[G_EVENTS];
     int launches = 0;
+    const char* kernels[G_COUNT];         // variant each group of the last pass ran (tsfx_last_kernels)
+    int n_kernels = 0;
     CsrWorkspace csr;
     ImputeWorkspace imp;
     SelectWorkspace sel;
@@ -622,6 +624,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
     const bool timing = (flags & TSFX_FLAG_TIMING) != 0;
     for (int g = 0; g < G_EVENTS; ++g) ctx->ev_used[g] = false;
     ctx->launches = 0;
+    ctx->n_kernels = 0;
     if (R.n_series == 0) return TSFX_OK;
     const int staged = P->cum[G_COUNT];
     if (staged == 0) return TSFX_OK;
@@ -659,6 +662,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         if (P->host[g].empty()) continue;
         if (timing) { CK(cudaEventRecord(ctx->ev[g][0], ctx->stream)); }
         cudaError_t e = cudaSuccess;
+        const char* variant = nullptr;
         double* d_out = (double*)ctx->stage.p + (size_t)R.n_series * P->cum[g];      // this group's staging matrix
         const int sidx = launched++ % nstreams;
         cudaStream_t gs = (sidx == 0) ? ctx->stream : ctx->s_side[sidx - 1];
@@ -678,7 +682,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                     M.out = direct ? d_final : d_out;
                     M.ncols = direct ? ld : g_ncols;
                     M.colmap = direct ? P->d_final_col + P->cum[g] : nullptr;
-                    e = launch_moments(M, gs, ctx->sm_count);
+                    e = launch_moments(M, gs, ctx->sm_count, &variant);
                     ctx->used_moments = true;
                     break;
                 }
@@ -700,7 +704,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                         }
                 }
                 A.dec = ctx->d_dec;
-                e = launch_basic(A, max_len, gs, ctx->sm_count);
+                e = launch_basic(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_SORTED: {
@@ -714,7 +718,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                     for (const Desc& q : P->host[g])
                         if (q.calc == TSFX_CHANGE_QUANTILES && !(q.p0 == pl && q.p1 == ph)) { ++A.ncq; pl = q.p0; ph = q.p1; }
                 }
-                e = launch_sorted(A, max_len, gs, ctx->sm_count);
+                e = launch_sorted(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_SPECTRAL: {
@@ -725,20 +729,20 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                 A.need_fft = P->need_fft; A.need_welch = P->need_welch;
                 A.max_hist = P->fourier_bins;
                 A.nfft = P->spectral_nfft;
-                e = launch_spectral(A, max_len, gs, ctx->sm_count);
+                e = launch_spectral(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_LA: {
                 LaArgs A;
                 A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
                 A.nscr = P->max_ar_k;
-                e = launch_la(A, max_len, gs, ctx->sm_count);
+                e = launch_la(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_ENTROPY: {
                 EntropyArgs A;
                 A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                e = launch_entropy(A, max_len, gs, ctx->sm_count);
+                e = launch_entropy(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_SEQ: {
@@ -746,7 +750,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                 A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
                 A.nscr = (P->max_lz_bins > 0 ? 1 : 0) | (P->max_perm_dim > 0 ? 2 : 0) | (P->max_cwt_peaks_n << 8) |
                          (std::min(P->n_lz, 255) << 16) | (std::min(P->max_lz_bins, 255) << 24);
-                e = launch_seq(A, max_len, gs, ctx->sm_count);
+                e = launch_seq(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
             case G_PEAKS: {
@@ -754,13 +758,14 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                 A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
                 A.nscr = (P->max_cwt_peaks_n << 8);
                 A.ricker = ctx->d_ricker;
-                e = launch_peaks(A, max_len, gs, ctx->sm_count);
+                e = launch_peaks(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
         }
         if (e == cudaErrorInvalidConfiguration) return too_long(kGroupNames[g]);
         if (e != cudaSuccess) return fail(ctx, TSFX_E_CUDA, std::string("launch ") + kGroupNames[g] + ": " + cudaGetErrorString(e));
         ctx->launches += 1;
+        ctx->kernels[ctx->n_kernels++] = variant;
         if (timing) { CK(cudaEventRecord(ctx->ev[g][1], ctx->stream)); ctx->ev_used[g] = true; }
     }
     if (nstreams > 1)
@@ -996,6 +1001,33 @@ extern "C" int tsfx_get_timings(tsfx_ctx* ctx, float* ms_out, const char** names
 }
 
 extern "C" int tsfx_last_launch_count(const tsfx_ctx* ctx) { return ctx ? ctx->launches : 0; }
+
+extern "C" int tsfx_last_kernels(const tsfx_ctx* ctx, const char** names_out, int32_t cap) {
+    if (!ctx || cap < 0 || (cap > 0 && !names_out)) return TSFX_E_INVALID;
+    const int k = std::min<int>(ctx->n_kernels, cap);
+    for (int i = 0; i < k; ++i) names_out[i] = ctx->kernels[i];
+    return k;
+}
+
+// every name a launcher can report (TSFX_GEOM_NAMES expands to the six plan_geometry placements of a kernel)
+#define TSFX_GEOM_LIST(GRP) GRP "/w8/shared", GRP "/w4/shared", GRP "/w2/shared", GRP "/w1/shared", GRP "/w4/global", GRP "/w1/global"
+static const char* const kKernelVariants[] = {
+    "moments/dense", "moments/general",
+    "basic/w12/shared", "basic/w24/shared", TSFX_GEOM_LIST("basic"),
+    "sorted/w12/shared", TSFX_GEOM_LIST("sorted"),
+    TSFX_GEOM_LIST("spectral"), TSFX_GEOM_LIST("spectral/pow2"),
+    TSFX_GEOM_LIST("la"),
+    "entropy/rank-g1", "entropy/rank-g4", "entropy/rank-g16", TSFX_GEOM_LIST("entropy/tiles"), TSFX_GEOM_LIST("entropy/pairs"),
+    "seq/small", TSFX_GEOM_LIST("seq/general"),
+    "peaks/small", TSFX_GEOM_LIST("peaks/general"), "peaks/general/hybrid/w4/global", "peaks/general/hybrid/w1/global",
+};
+#undef TSFX_GEOM_LIST
+
+extern "C" int tsfx_kernel_variants(const char** names_out, int32_t cap) {
+    const int n = (int)(sizeof(kKernelVariants) / sizeof(kKernelVariants[0]));
+    for (int i = 0; i < n && i < cap && names_out; ++i) names_out[i] = kKernelVariants[i];
+    return n;
+}
 
 // ------------------------------------------------------------------------------------------ stage (a)
 // Long frame -> device CSR -> kernels, pipelined.  See tsfx_csr.h for the two paths.  `in` columns are host pointers

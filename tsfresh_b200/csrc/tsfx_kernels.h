@@ -17,21 +17,23 @@ int global_ctas_env();
 struct Geometry { int wpc; size_t smem; int grid; unsigned char* gscratch; };
 
 // Chooses warps per CTA / grid for a warp-per-series kernel needing `per` bytes per warp.  Shared memory when it
-// fits (budget = target bytes per CTA so several CTAs stay resident), else the global scratch buffer.
+// fits (budget = target bytes per CTA so several CTAs stay resident), else the global scratch buffer.  `cta_bytes` of
+// shared memory in front of the per-warp regions are needed in either placement (k_basic's descriptor table): they
+// count against the 227 KB of one CTA, and G->smem includes them.
 inline bool plan_geometry(size_t per, size_t budget, int maxw, int64_t n_series, int sm_count, unsigned char* gs,
                           size_t gs_bytes, Geometry* G, size_t prefer_global_above = 227 * 1024,
-                          int global_ctas = 0) {
+                          int global_ctas = 0, size_t cta_bytes = 0) {
     // Working sets above `prefer_global_above` bytes per warp run from the global (L2-resident) region even though
     // they would fit in shared memory: shared memory would limit the latency-bound PEAKS / SEQ kernels to 2-4 warps per
     // SM -- measured on H100 SXM (700 W) at 250 000 x 1024, PEAKS 61 ms against 266 ms, SEQ 67 ms against 143 ms.
     // TSFX_GLOBAL_ABOVE=<bytes> overrides the per-kernel threshold for experiments.
     const size_t thr = global_above() > 0 ? (size_t)global_above() : prefer_global_above;
-    if (per <= thr && per <= 227 * 1024) {
+    if (per <= thr && per + cta_bytes <= 227 * 1024) {
         size_t w = budget / per;
         int wpc = w >= 8 ? 8 : w >= 4 ? 4 : w >= 2 ? 2 : 1;
         while (wpc > maxw) wpc >>= 1;
         G->wpc = wpc;
-        G->smem = per * wpc;
+        G->smem = per * wpc + cta_bytes;
         int64_t cap = (int64_t)sm_count * grid_waves(4096);
         int64_t ctas = (n_series + wpc - 1) / wpc;
         G->grid = (int)(ctas < cap ? (ctas < 1 ? 1 : ctas) : cap);
@@ -47,10 +49,19 @@ inline bool plan_geometry(size_t per, size_t budget, int maxw, int64_t n_series,
     int64_t cap = (int64_t)sm_count * (global_ctas_env() > 0 ? global_ctas_env() : global_ctas > 0 ? global_ctas : 4);
     if ((int64_t)max_ctas < cap) cap = (int64_t)max_ctas;
     G->wpc = wpc;
-    G->smem = 0;
+    G->smem = cta_bytes;
     G->grid = (int)(ctas < cap ? (ctas < 1 ? 1 : ctas) : cap);
     G->gscratch = gs;
     return true;
+}
+
+// Variant names reported by tsfx_last_kernels: "<group>/w<warps per CTA>/<shared | global>" for the plan_geometry
+// kernels.  Every name any launcher can report is listed in kKernelVariants (tsfx_api.cu).
+#define TSFX_GEOM_NAMES(GRP) \
+    { GRP "/w8/shared", GRP "/w4/shared", GRP "/w2/shared", GRP "/w1/shared", GRP "/w4/global", GRP "/w1/global" }
+inline const char* geom_variant(const char* const (&names)[6], const Geometry& G) {
+    if (G.gscratch) return names[G.wpc == 4 ? 4 : 5];
+    return names[G.wpc == 8 ? 0 : G.wpc == 4 ? 1 : G.wpc == 2 ? 2 : 3];
 }
 
 #define TSFX_LAUNCH_GEOM(KERNEL, W, GS, G, st, ...)                                                               \
@@ -114,7 +125,7 @@ struct BasicArgs {
     int pacf_off;        // offset (doubles) of the pacf staging area inside lagS
     const double* dec;   // device table d*10^k, k = TSFX_DEC_MIN..TSFX_DEC_MAX, 9 per decade
 };
-cudaError_t launch_basic(const BasicArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_basic(const BasicArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 bool basic_finisher_calc(int calc);
 bool sorted_finisher_calc(int calc);    // same for the SORTED group     // host: is this calculator evaluated by the lane-parallel finisher stage?
 
@@ -128,7 +139,7 @@ struct MomentsArgs {
     const int32_t* colmap;   // device: final column of descriptor j (direct write, no assemble pass), or nullptr
     int need_high;       // third / fourth centred moments are needed (skewness, kurtosis)
 };
-cudaError_t launch_moments(const MomentsArgs& A, cudaStream_t st, int sm_count);
+cudaError_t launch_moments(const MomentsArgs& A, cudaStream_t st, int sm_count, const char** variant);
 bool moments_only_calc(int calc);       // host: can the reduction-only kernel evaluate this calculator?
 
 struct SortedArgs {
@@ -142,7 +153,7 @@ struct SortedArgs {
     int npad, npow2, nscr, bytes_per_warp;
     int nfin, ncq;       // leading O(1) descriptors (lane-parallel); distinct change_quantiles corridors
 };
-cudaError_t launch_sorted(const SortedArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_sorted(const SortedArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct SpectralArgs {
     SeriesRef R;
@@ -162,7 +173,7 @@ struct SpectralArgs {
     int max_hist;
     int nfft;                  // the first nfft descriptors are fft_coefficient (lane-parallel stage)
 };
-cudaError_t launch_spectral(const SpectralArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_spectral(const SpectralArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct LaArgs {
     SeriesRef R;
@@ -174,7 +185,7 @@ struct LaArgs {
     int ncols;
     int npad, nscr, bytes_per_warp;
 };
-cudaError_t launch_la(const LaArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_la(const LaArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct EntropyArgs {
     int rank_pad;              // rank-space kernel: pad the prefix-table rows (bank conflicts vs. occupancy)
@@ -188,7 +199,7 @@ struct EntropyArgs {
     int ncols;
     int npad, bytes_per_warp;
 };
-cudaError_t launch_entropy(const EntropyArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_entropy(const EntropyArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct SeqArgs {
     SeriesRef R;
@@ -201,8 +212,8 @@ struct SeqArgs {
     int npad, nscr, bytes_per_warp;
     const double* ricker = nullptr;    // PEAKS: device Ricker tap table (launch_fill_ricker)
 };
-cudaError_t launch_seq(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count);
-cudaError_t launch_peaks(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count);
+cudaError_t launch_seq(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
+cudaError_t launch_peaks(const SeqArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 // Ricker tap table of number_cwt_peaks: widths 1..TSFX_RICKER_W, entry (w - 1) * TSFX_RICKER_K + |2 v - (points - 1)|
 // is tap v of ricker(points, w) for every points <= 10 w (filled once per context, on the device)
