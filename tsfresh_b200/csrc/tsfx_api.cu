@@ -1016,7 +1016,7 @@ static const char* const kKernelVariants[] = {
     "basic/w12/shared", "basic/w24/shared", TSFX_GEOM_LIST("basic"),
     "sorted/w12/shared", TSFX_GEOM_LIST("sorted"),
     TSFX_GEOM_LIST("spectral"), TSFX_GEOM_LIST("spectral/pow2"),
-    TSFX_GEOM_LIST("la"),
+    "la/small", TSFX_GEOM_LIST("la"),
     "entropy/rank-g1", "entropy/rank-g4", "entropy/rank-g16", TSFX_GEOM_LIST("entropy/tiles"), TSFX_GEOM_LIST("entropy/pairs"),
     "seq/small", TSFX_GEOM_LIST("seq/general"),
     "peaks/small", TSFX_GEOM_LIST("peaks/general"), "peaks/general/hybrid/w4/global", "peaks/general/hybrid/w1/global",
