@@ -8,8 +8,8 @@ targets; the bounds in BOUNDS are the lengths at which the choice changes for th
   * boundary sweep: one plan per kernel group, the series that selects the variant next to short and degenerate series
     (1-5, 8, 31-33 and 255 samples, constant, tied), CSR and dense input;
   * long series: ComprehensiveFCParameters at 11 300, 12 000 and 21 000 samples; 21 001 is TSFX_E_TOO_LONG;
-  * forced variants: the launch knobs (read once per process) in subprocesses -- global-region instantiations, the
-    entropy tile kernel in shared memory and in the global region, four streams;
+  * forced variants: the launch knobs (read once per process) in subprocesses -- global-region instantiations, among
+    them the entropy tile kernel's, and four streams;
   * warp reuse: a grid of one CTA (wave) per SM, so every warp processes many series in turn, must give the same bits as
     batches in which no warp processes two series; permuting the rows permutes the result;
   * ledger: every variant the launchers can choose under the default and the tested settings was reported here.
@@ -282,13 +282,15 @@ def test_longer_than_21000_is_too_long(ctx):
 
 # ---------------------------------------------------------------------------------------------- forced variants
 def _forced_cases():
-    """(name, settings, series, dense, degenerate rows): Comprehensive at 256 and 1000 samples next to the short and
-    degenerate series, the SPECTRAL group on dense power-of-two rows"""
+    """(name, settings, series, dense, degenerate rows): Comprehensive at 256 and 1000 samples and the ENTROPY group at
+    1200 samples (the tile kernel) next to the short and degenerate series, the SPECTRAL group on dense power-of-two rows"""
     cases = []
-    for length in (256, 1000):
-        extra = short_and_degenerate("basic", seed=length + 1)
-        cases.append(("comprehensive_%d" % length, ComprehensiveFCParameters(),
-                      main_series(length, length + 2) + [s for s, _ in extra], False, [False, False] + [d for _, d in extra]))
+    for name, settings, group, length in (("comprehensive_256", ComprehensiveFCParameters(), "basic", 256),
+                                          ("comprehensive_1000", ComprehensiveFCParameters(), "basic", 1000),
+                                          ("entropy_1200", group_settings("entropy"), "entropy", 1200)):
+        extra = short_and_degenerate(group, seed=length + 1)
+        cases.append((name, settings, main_series(length, length + 2) + [s for s, _ in extra], False,
+                      [False, False] + [d for _, d in extra]))
     rng = np.random.default_rng(4)
     cases.append(("spectral_dense_256", group_settings("spectral"),
                   [rng.standard_normal(256).astype(np.float32) for _ in range(4)], True, [False] * 4))
@@ -353,45 +355,39 @@ def _in_subprocess(tmp_path, what, tag, env):
     return {k: arrays[k] for k in arrays.files}, kernels
 
 
-FORCED = {       # configuration -> (environment, variants it must reach, entropy kernel differs from the default)
-    "default": ({}, set(), False),
+FORCED = {       # configuration -> (environment, variants it must reach)
+    "default": ({}, {"entropy/tiles/w2/shared"}),
     "global": ({"TSFX_GLOBAL_ABOVE": "1"},
-               {"basic/w4/global", "sorted/w4/global", "spectral/w4/global", "la/w4/global", "spectral/pow2/w4/global"}, False),
-    "tiles": ({"TSFX_ENTROPY": "t"}, {"entropy/tiles/w4/shared", "entropy/tiles/w2/shared"}, True),
-    "tiles_global": ({"TSFX_ENTROPY": "t", "TSFX_GLOBAL_ABOVE": "1"}, {"entropy/tiles/w4/global"}, True),
-    "streams": ({"TSFX_STREAMS": "4"}, set(), False),
+               {"basic/w4/global", "sorted/w4/global", "spectral/w4/global", "la/w4/global", "spectral/pow2/w4/global",
+                "entropy/tiles/w4/global"}),
+    "streams": ({"TSFX_STREAMS": "4"}, set()),
 }
 
 
 def test_forced_variants(pool, tmp_path):
-    """Every configuration matches the oracle.  Those that change only where the working set lives, the warps per CTA
-    or the stream a group runs on give the default's bits; the tile kernel counts the same template matches as the
-    rank kernel but sums the logarithms of approximate_entropy in another order, so its ENTROPY columns are compared with
-    the oracle only -- and the tile kernel in the global region gives the same bits as in shared memory."""
+    """Every configuration matches the oracle, and gives the default's bits: they change only where the working set
+    lives, the warps per CTA or the stream a group runs on."""
     cases = _forced_cases()
     want = {name: oracle(pool, settings, series) for name, settings, series, _, _ in cases}
-    res = {cfg: _in_subprocess(tmp_path, "forced", cfg, env) for cfg, (env, _, _) in FORCED.items()}
+    res = {cfg: _in_subprocess(tmp_path, "forced", cfg, env) for cfg, (env, _) in FORCED.items()}
     failures = []
-    for cfg, (env, must, entropy_differs) in FORCED.items():
+    for cfg, (env, must) in FORCED.items():
         got, kernels = res[cfg]
         reached = {k for v in kernels.values() for k in v}
         if not must <= reached:
             failures.append("%s: did not reach %s (ran %s)" % (cfg, sorted(must - reached), sorted(reached)))
-        ref = res["tiles" if cfg == "tiles_global" else "default"][0]
+        ref = res["default"][0]
         for name, settings, series, dense, degenerate in cases:
             suffixes = Plan(settings).suffixes
             bad = check(got[name], want[name], suffixes, degenerate)
             if bad:
                 failures.append("%s / %s vs oracle:\n%s" % (cfg, name, _report(bad)))
-            cols = [c for c, s in enumerate(suffixes)
-                    if not (entropy_differs and cfg != "tiles_global" and s.split("__")[0] in _CALCS["entropy"])]
-            a, b = got[name][:, cols], ref[name][:, cols]
+            a, b = got[name], ref[name]
             diff = ~((a == b) | (np.isnan(a) & np.isnan(b)))
             if diff.any():
                 r, c = np.argwhere(diff)[0]
-                failures.append("%s / %s: %d cells differ from %s, first row %d %s: %r vs %r" % (
-                    cfg, name, diff.sum(), "tiles" if cfg == "tiles_global" else "default", r,
-                    suffixes[cols[c]], a[r, c], b[r, c]))
+                failures.append("%s / %s: %d cells differ from default, first row %d %s: %r vs %r" % (
+                    cfg, name, diff.sum(), r, suffixes[c], a[r, c], b[r, c]))
     assert not failures, "\n".join(failures)
 
 
@@ -452,24 +448,11 @@ def test_row_permutation(ctx, name):
 
 
 # ---------------------------------------------------------------------------------------------- ledger
-# variants no test here can reach: chosen only by the A/B tuning variables, or never by the sizes run_groups gives the
-# global working region (256 MB up to 1 024 samples, 1 GB beyond: four warps' working sets always fit)
-NOT_REACHED = {
-    "basic/w24/shared": "TSFX_BASIC_WPC=24",
-    "basic/w8/shared": "TSFX_BASIC_WPC=8 (8-warp geometries otherwise run as 12-warp CTAs)",
-    "sorted/w12/shared": "TSFX_SORTED_WPC=12",
-}
-NOT_REACHED.update({"entropy/pairs/" + p: "TSFX_ENTROPY=p" for p in ("w8/shared", "w4/shared", "w2/shared", "w1/shared",
-                                                                      "w4/global", "w1/global")})
-NOT_REACHED.update({g + "/w1/global": "the global working region always holds four warps"
-                    for g in ("basic", "sorted", "spectral", "spectral/pow2", "la", "entropy/tiles", "seq/general",
-                              "peaks/general", "peaks/general/hybrid")})
-NOT_REACHED.update({"entropy/tiles/w8/shared": "the tile kernel runs at most 4 warps per CTA"})
-NOT_REACHED.update({"seq/general/w2/shared": "the general SEQ kernel leaves shared memory above 16 KB per warp (>= 4 warps)",
-                    "seq/general/w1/shared": "the general SEQ kernel leaves shared memory above 16 KB per warp (>= 4 warps)"})
-NOT_REACHED.update({"peaks/general/" + p: "series the compact PEAKS kernel does not take need more than the 16 KB per warp "
-                    "below which the general kernel stays in shared memory (TSFX_GLOBAL_ABOVE can raise that bound)"
-                    for p in ("w8/shared", "w4/shared", "w2/shared", "w1/shared")})
+# variants no test here can reach: never chosen at the sizes run_groups gives the global working region (256 MB up to
+# 1 024 samples, 1 GB beyond: four warps' working sets always fit)
+NOT_REACHED = {g + "/w1/global": "the global working region always holds four warps"
+               for g in ("basic", "sorted", "spectral", "spectral/pow2", "la", "entropy/tiles", "seq/general",
+                         "peaks/general", "peaks/general/hybrid")}
 
 
 def test_variant_ledger(request):

@@ -894,16 +894,14 @@ bool basic_finisher_calc(int calc) { return basic_is_finisher(calc); }
 
 // ------------------------------------------------------------------------------------------ launcher
 cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
-    static const char* const names[6] = TSFX_GEOM_NAMES("basic");
     BasicArgs A = A0;
     A.npad = (max_len + 3) & ~3;
+    A.nscr = std::max(A.nscr, (max_len + 1) & ~1);      // the plan's scratch need, at least the series
     A.nxc = ((max_len + 255) / 256) * 256 + ((A.lag_needed + 1) & ~1);      // centred copy + zero tail for the lag products
     {
-        // lag products on the FP64 tensor cores (DMMA) unless TSFX_LAG=fma or the largest lag needs more than 8 tiles
-        static int mode = -1;
-        if (mode < 0) { const char* e = getenv("TSFX_LAG"); mode = (e && e[0] == 'f') ? 0 : 1; }
+        // lag products on the FP64 tensor cores (DMMA) unless the largest lag needs more than 8 tiles
         const int tiles = A.lag_needed / 8 + 1 + ((A.lag_needed & 7) ? 1 : 0);
-        A.lag_tiles = (mode == 1 && A.lag_needed > 0 && tiles <= TSFX_DMMA_MAX_TILES) ? tiles : 0;
+        A.lag_tiles = (A.lag_needed > 0 && tiles <= TSFX_DMMA_MAX_TILES) ? tiles : 0;
         if (A.lag_tiles > 0) {     // the strided fragment loads read up to 32 ceil(n / 32) + 8 tiles + 24 samples
             const int need = ((max_len + 31) / 32) * 32 + 8 * A.lag_tiles + 32;
             if (A.nxc < need) A.nxc = (need + 1) & ~1;
@@ -919,36 +917,17 @@ cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int 
     if (!plan_geometry(per, budget, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G, 227 * 1024, 0, A.desc_bytes))
         return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    {
-        // Two CTAs of 12 warps per SM instead of three of 8 (TSFX_BASIC_WPC=8|12|24): all warps of a CTA walk the descriptor
-        // list in lock step, so larger CTAs share more of the 250 KB instruction stream -- measured on H100 SXM (700 W) at
-        // 1 M x 256: 56.5 ms (3 x 8) -> 49.7 ms (2 x 12), 51.0 ms (1 x 24)
-        static int wide = -1;
-        if (wide < 0) { const char* e = getenv("TSFX_BASIC_WPC"); wide = e ? atoi(e) : 12; }
-        if ((wide == 12 || wide == 24) && !G.gscratch && G.wpc == 8) {
-            const size_t smem = per * wide + A.desc_bytes;
-            if (smem <= 227 * 1024) {
-                const int64_t ctas = (A.R.n_series + wide - 1) / wide;
-                const int64_t cap = (int64_t)sm_count * grid_waves(4096);
-                const int grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
-                cudaError_t e;
-                *variant = wide == 12 ? "basic/w12/shared" : "basic/w24/shared";
-                if (wide == 12) {
-                    e = cudaFuncSetAttribute(k_basic<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    if (e != cudaSuccess) return e;
-                    k_basic<12, false><<<grid, 12 * 32, smem, st>>>(A);
-                } else {
-                    e = cudaFuncSetAttribute(k_basic<24, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-                    if (e != cudaSuccess) return e;
-                    k_basic<24, false><<<grid, 24 * 32, smem, st>>>(A);
-                }
-                return cudaGetLastError();
-            }
-        }
+    if (!G.gscratch && G.wpc == 8) {
+        // Two CTAs of 12 warps per SM instead of three of 8: all warps of a CTA walk the descriptor list in lock step, so
+        // larger CTAs share more of the 250 KB instruction stream -- measured on H100 SXM (700 W) at 1 M x 256: 56.5 ms
+        // (3 x 8) -> 49.7 ms (2 x 12), 51.0 ms (1 x 24).  Eight warps fit the budget, 8 per + desc_bytes <= 100 KB, so
+        // 12 per + desc_bytes <= 150 KB: twelve always fit one CTA's 227 KB.
+        G.wpc = 12;
+        G.smem = per * 12 + A.desc_bytes;
+        G.grid = cta_grid(A.R.n_series, 12, (int64_t)sm_count * grid_waves(4096));
     }
-    *variant = geom_variant(names, G);
-    TSFX_DISPATCH(k_basic, G, st, A)
-    return cudaGetLastError();
+    auto launch = [&](auto g) { return launch_kernel(k_basic<decltype(g)::wpc, decltype(g)::global>, G, st, A); };
+    TSFX_LAUNCH_DECLARED(TSFX_GEOMS_BASIC, "basic", G, variant, launch);
 }
 
 }  // namespace tsfx

@@ -638,26 +638,18 @@ __global__ void __launch_bounds__(WPC * 32, MINB) k_la_small(LaArgs A) {
 }
 
 cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
-    static const char* const names[6] = TSFX_GEOM_NAMES("la");
-    if (max_len <= LA_SMALL_LEN && A0.nscr <= LA_SMALL_KMAX) {
-        LaArgs A = A0;
+    LaArgs A = A0;
+    if (max_len <= LA_SMALL_LEN && A.max_ar_k <= LA_SMALL_KMAX) {
         A.npad = LA_SMALL_LEN;
         A.bytes_per_warp = (LA_SMALL_LEN + LA_SMALL_P * LA_SMALL_LD + LA_SMALL_CB + 32) * 8;
         A.gscratch = nullptr;
-        const size_t smem = (size_t)A.bytes_per_warp * LA_SMALL_WPC;
-        const int64_t ctas = (A.R.n_series + LA_SMALL_WPC - 1) / LA_SMALL_WPC;
-        const int64_t cap = (int64_t)sm_count * grid_waves(4096);
-        const int grid = (int)std::max<int64_t>(1, std::min(ctas, cap));
         *variant = "la/small";
-        cudaError_t e = cudaFuncSetAttribute(k_la_small<LA_SMALL_WPC, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        k_la_small<LA_SMALL_WPC, 3><<<grid, LA_SMALL_WPC * 32, smem, st>>>(A);
-        return cudaGetLastError();
+        return launch_fixed(k_la_small<LA_SMALL_WPC, 3>, LA_SMALL_WPC * 32, LA_SMALL_WPC, (size_t)A.bytes_per_warp * LA_SMALL_WPC,
+                            (int64_t)sm_count * grid_waves(4096), A.R.n_series, st, A);
     }
-    LaArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     if (adf_maxlag(max_len) + 2 > 64) return cudaErrorInvalidConfiguration;     // autolag keeps one model per lane, two rounds
-    int pmax = std::max(adf_maxlag(max_len) + 2, A.nscr + 1);   // nscr carries the plan's largest AR order k
+    int pmax = std::max(adf_maxlag(max_len) + 2, A.max_ar_k + 1);
     pmax = (pmax + 1) & ~1;
     size_t per = (size_t)A.npad * 16 + (size_t)pmax * pmax * 16 + (size_t)pmax * 24 + 64 + (size_t)A.npad * 4;
     per = (per + 15) & ~(size_t)15;
@@ -665,9 +657,8 @@ cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_cou
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    *variant = geom_variant(names, G);
-    TSFX_DISPATCH(k_la, G, st, A, pmax)
-    return cudaGetLastError();
+    auto launch = [&](auto g) { return launch_kernel(k_la<decltype(g)::wpc, decltype(g)::global>, G, st, A, pmax); };
+    TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "la", G, variant, launch);
 }
 
 }  // namespace tsfx

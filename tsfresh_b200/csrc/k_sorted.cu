@@ -404,38 +404,19 @@ bool sorted_finisher_calc(int calc) {
 }
 
 cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
-    static const char* const names[6] = TSFX_GEOM_NAMES("sorted");
     SortedArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     int p2 = 1;
     while (p2 < max_len) p2 <<= 1;
     A.npow2 = std::max(p2, 4);
-    A.nscr = (A.nscr + 1) & ~1;
     size_t per = (size_t)A.nscr * 8 + (size_t)(5 * A.ncq + (A.ncq & 1)) * 8 + (size_t)A.npad * 4 + (size_t)A.npow2 * 4;
     per = (per + 15) & ~(size_t)15;
     A.bytes_per_warp = (int)per;
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    {
-        // TSFX_SORTED_WPC=12: two CTAs of 12 warps per SM instead of three of 8 (same idea as k_basic: the lock-step walk
-        // shares the instruction stream inside a CTA)
-        static int wide = -1;
-        if (wide < 0) { const char* e = getenv("TSFX_SORTED_WPC"); wide = e ? atoi(e) : 0; }
-        if (wide == 12 && !G.gscratch && G.wpc == 8 && per * 12 <= 113 * 1024) {
-            const size_t smem = per * 12;
-            const int64_t ctas = (A.R.n_series + 11) / 12;
-            const int64_t cap = (int64_t)sm_count * grid_waves(4096);
-            *variant = "sorted/w12/shared";
-            cudaError_t e = cudaFuncSetAttribute(k_sorted<12, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-            if (e != cudaSuccess) return e;
-            k_sorted<12, false><<<(int)std::max<int64_t>(1, std::min(ctas, cap)), 12 * 32, smem, st>>>(A);
-            return cudaGetLastError();
-        }
-    }
-    *variant = geom_variant(names, G);
-    TSFX_DISPATCH(k_sorted, G, st, A)
-    return cudaGetLastError();
+    auto launch = [&](auto g) { return launch_kernel(k_sorted<decltype(g)::wpc, decltype(g)::global>, G, st, A); };
+    TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "sorted", G, variant, launch);
 }
 
 }  // namespace tsfx

@@ -308,8 +308,6 @@ __global__ void __launch_bounds__(WPC * 32) k_spectral(SpectralArgs A, int nwtab
 }
 
 cudaError_t launch_spectral(const SpectralArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
-    static const char* const names[6] = TSFX_GEOM_NAMES("spectral");
-    static const char* const names_pow2[6] = TSFX_GEOM_NAMES("spectral/pow2");     // dense power-of-two length: no twiddle-word table
     SpectralArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     A.nspec = A.npad / 2 + 2;
@@ -322,9 +320,10 @@ cudaError_t launch_spectral(const SpectralArgs& A0, int max_len, cudaStream_t st
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    *variant = geom_variant(dense_pow2 ? names_pow2 : names, G);
-    TSFX_DISPATCH(k_spectral, G, st, A, nwtab, nhist)
-    return cudaGetLastError();
+    auto launch = [&](auto g) { return launch_kernel(k_spectral<decltype(g)::wpc, decltype(g)::global>, G, st, A, nwtab, nhist); };
+    if (dense_pow2)          // dense power-of-two length: no twiddle-word table
+        TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "spectral/pow2", G, variant, launch);
+    TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "spectral", G, variant, launch);
 }
 
 }  // namespace tsfx

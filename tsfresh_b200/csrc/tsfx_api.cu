@@ -42,6 +42,12 @@ int global_ctas_env() {
     if (v < 0) { const char* e = getenv("TSFX_GLOBAL_CTAS"); v = e ? atoi(e) : 0; if (v < 1 || v > 16) v = 0; }
     return v;
 }
+cudaError_t undeclared_geometry(const char* grp, const Geometry& G, const char** variant) {
+    static thread_local std::string name;
+    name = std::string(grp) + "/w" + std::to_string(G.wpc) + (G.gscratch ? "/global" : "/shared");
+    *variant = name.c_str();
+    return cudaErrorNotSupported;
+}
 }  // namespace tsfx
 
 static int env_streams() {
@@ -274,18 +280,17 @@ struct tsfx_plan {
     bool basic_moments_only = false;  // the BASIC group is reductions only: k_moments replaces k_basic
     int moments_need_high = 0;
     int n_groups_used = 0;
-    int basic_nfin = 0;               // leading "finisher" descriptors of the BASIC group
-    int sorted_nfin = 0;              // same for the SORTED group
-    int spectral_nfft = 0;            // leading fft_coefficient descriptors of the SPECTRAL group
     int cum[G_COUNT + 1] = {0};
     int ncols = 0;
-    int lag_needed = 0, pacf_want = -1;
-    int basic_bins = 0, fourier_bins = 0;
-    int need_fft = 0, need_welch = 0;
-    int max_ar_k = 0, need_adf = 0;
-    int max_lz_bins = 0, max_perm_dim = 0, max_cwt_peaks_n = 0, n_lz = 0;
     int need_times = 0;               // linear_trend_timewise columns: the extract call needs tsfx_set_row_times
-    int friedrich_r = 0;
+    // each group's kernel arguments as far as the plan fixes them (run_groups adds the call's series and buffers)
+    BasicArgs basic = {};
+    SortedArgs sorted = {};
+    SpectralArgs spectral = {};
+    LaArgs la = {};
+    EntropyArgs entropy = {};
+    SeqArgs seq = {};
+    PeaksArgs peaks = {};
     double* d_tables = nullptr;
     int64_t* d_toff = nullptr;
     int32_t* d_thalf = nullptr;
@@ -429,6 +434,8 @@ extern "C" int tsfx_sync(tsfx_ctx* ctx) {
 }
 
 // ------------------------------------------------------------------------------------------ plan
+static int even(int v) { return (v + 1) & ~1; }
+
 extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, int32_t n_descs, int32_t n_cols,
                                 const double* tables, const int64_t* table_off, const int32_t* table_half,
                                 int32_t n_tables, tsfx_plan** out) {
@@ -441,6 +448,9 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
     if (!P) return fail(ctx, TSFX_E_NOMEM, "out of host memory");
     P->ctx = ctx;
     P->ncols = n_cols;
+    int lag_needed = 0, pacf_want = -1, basic_bins = 0, fourier_bins = 0, need_fft = 0, need_welch = 0, max_ar_k = 0;
+    int max_lz_bins = 0, max_perm_dim = 0, max_cwt_peaks_n = 0, n_lz = 0, friedrich_r = 0;
+    int basic_nfin = 0, sorted_nfin = 0, spectral_nfft = 0;     // leading finisher / fft_coefficient descriptors
     for (int i = 0; i < n_descs; ++i) {
         const Desc& d = descs[i];
         if (d.calc < 0 || d.calc >= TSFX_N_CALCS || d.col < 0 || d.col >= n_cols) {
@@ -449,45 +459,44 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         }
         P->host[group_of(d.calc)].push_back(d);
         switch (d.calc) {
-            case TSFX_AUTOCORRELATION: P->lag_needed = std::max(P->lag_needed, d.i0); break;
-            case TSFX_AGG_AUTOCORRELATION: P->lag_needed = std::max(P->lag_needed, d.i0); break;
+            case TSFX_AUTOCORRELATION: lag_needed = std::max(lag_needed, d.i0); break;
+            case TSFX_AGG_AUTOCORRELATION: lag_needed = std::max(lag_needed, d.i0); break;
             case TSFX_PARTIAL_AUTOCORRELATION:
-                P->lag_needed = std::max(P->lag_needed, d.i1);
-                P->pacf_want = std::max(P->pacf_want, d.i1);
+                lag_needed = std::max(lag_needed, d.i1);
+                pacf_want = std::max(pacf_want, d.i1);
                 break;
-            case TSFX_BINNED_ENTROPY: P->basic_bins = std::max(P->basic_bins, d.i0); break;
-            case TSFX_FOURIER_ENTROPY: P->fourier_bins = std::max(P->fourier_bins, d.i0); P->need_welch = 1; break;
-            case TSFX_SPKT_WELCH_DENSITY: P->need_welch = 1; break;
-            case TSFX_FFT_COEFFICIENT: case TSFX_FFT_AGGREGATED: P->need_fft = 1; break;
+            case TSFX_BINNED_ENTROPY: basic_bins = std::max(basic_bins, d.i0); break;
+            case TSFX_FOURIER_ENTROPY: fourier_bins = std::max(fourier_bins, d.i0); need_welch = 1; break;
+            case TSFX_SPKT_WELCH_DENSITY: need_welch = 1; break;
+            case TSFX_FFT_COEFFICIENT: case TSFX_FFT_AGGREGATED: need_fft = 1; break;
             case TSFX_CWT_COEFFICIENTS:
                 if (d.i1 < 0 || d.i1 >= n_tables) { delete P; return fail(ctx, TSFX_E_INVALID, "cwt table index out of range"); }
                 break;
             case TSFX_AR_COEFFICIENT:
                 if (d.i1 < 1 || d.i1 > 32) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "ar_coefficient: k must be in 1..32"); }
-                P->max_ar_k = std::max(P->max_ar_k, d.i1);
+                max_ar_k = std::max(max_ar_k, d.i1);
                 break;
-            case TSFX_AUGMENTED_DICKEY_FULLER: P->need_adf = 1; break;
             case TSFX_LINEAR_TREND_TIMEWISE: P->need_times = 1; break;
             case TSFX_APPROXIMATE_ENTROPY:
                 if (d.i0 != 2) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "approximate_entropy: only m=2"); }
                 break;
-            case TSFX_LEMPEL_ZIV_COMPLEXITY: P->max_lz_bins = std::max(P->max_lz_bins, d.i0); P->n_lz += 1; break;
+            case TSFX_LEMPEL_ZIV_COMPLEXITY: max_lz_bins = std::max(max_lz_bins, d.i0); n_lz += 1; break;
             case TSFX_PERMUTATION_ENTROPY:
                 if (d.i1 < 2 || d.i1 > 8 || d.i0 < 1) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "permutation_entropy: dimension 2..8, tau >= 1"); }
-                P->max_perm_dim = std::max(P->max_perm_dim, d.i1);
+                max_perm_dim = std::max(max_perm_dim, d.i1);
                 break;
             case TSFX_NUMBER_CWT_PEAKS:
                 if (d.i0 < 1 || d.i0 > 16) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "number_cwt_peaks: n must be in 1..16"); }
-                P->max_cwt_peaks_n = std::max(P->max_cwt_peaks_n, d.i0);
+                max_cwt_peaks_n = std::max(max_cwt_peaks_n, d.i0);
                 break;
             case TSFX_FRIEDRICH_COEFFICIENTS: case TSFX_MAX_LANGEVIN_FIXED_POINT:
                 if (d.i1 != 3 || d.i2 < 1 || d.i2 > 256) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "friedrich: only m=3, r in 1..256"); }
-                P->friedrich_r = std::max(P->friedrich_r, d.i2);
+                friedrich_r = std::max(friedrich_r, d.i2);
                 break;
             default: break;
         }
     }
-    if (P->lag_needed > 4096) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "lag > 4096"); }
+    if (lag_needed > 4096) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "lag > 4096"); }
     std::vector<int32_t> final_col;
     for (int g = 0; g < G_COUNT; ++g) {
         std::stable_sort(P->host[g].begin(), P->host[g].end(), [g](const Desc& a, const Desc& b) {
@@ -513,11 +522,11 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
             return a.col < b.col;
         });
         if (g == G_BASIC)
-            for (const Desc& d : P->host[g]) P->basic_nfin += basic_finisher_calc(d.calc) ? 1 : 0;
+            for (const Desc& d : P->host[g]) basic_nfin += basic_finisher_calc(d.calc) ? 1 : 0;
         if (g == G_SORTED)
-            for (const Desc& d : P->host[g]) P->sorted_nfin += sorted_finisher_calc(d.calc) ? 1 : 0;
+            for (const Desc& d : P->host[g]) sorted_nfin += sorted_finisher_calc(d.calc) ? 1 : 0;
         if (g == G_SPECTRAL)
-            for (const Desc& d : P->host[g]) P->spectral_nfft += (d.calc == TSFX_FFT_COEFFICIENT) ? 1 : 0;
+            for (const Desc& d : P->host[g]) spectral_nfft += (d.calc == TSFX_FFT_COEFFICIENT) ? 1 : 0;
         P->cum[g + 1] = P->cum[g] + (int)P->host[g].size();
         for (size_t j = 0; j < P->host[g].size(); ++j) {      // col becomes the index inside the group's staging row
             final_col.push_back(P->host[g][j].col);
@@ -535,7 +544,6 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         if (!moments_only_calc(d.calc)) P->basic_moments_only = false;
         if (d.calc == TSFX_SKEWNESS || d.calc == TSFX_KURTOSIS) P->moments_need_high = 1;
     }
-    { const char* e = getenv("TSFX_NO_MOMENTS_KERNEL"); if (e && e[0] == '1') P->basic_moments_only = false; }
     for (int g = 0; g < G_COUNT; ++g) P->n_groups_used += P->host[g].empty() ? 0 : 1;
     if (!final_col.empty()) {
         cudaError_t e = cudaMalloc(&P->d_final_col, final_col.size() * sizeof(int32_t));
@@ -556,6 +564,42 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         if (e == cudaSuccess) e = cudaMemcpy(P->d_thalf, table_half, n_tables * sizeof(int32_t), cudaMemcpyHostToDevice);
         if (e != cudaSuccess) { tsfx_plan_destroy(P); return fail(ctx, TSFX_E_CUDA, cudaGetErrorString(e)); }
     }
+    auto group = [&](GroupArgs& A, int g) { A.descs = P->dev[g]; A.nd = A.ncols = (int)P->host[g].size(); };
+    BasicArgs& B = P->basic;
+    group(B, G_BASIC);
+    B.lag_needed = lag_needed;
+    B.nfin = basic_nfin;
+    B.pacf_off = lag_needed + 1;
+    B.nlag = even(lag_needed + 1 + (pacf_want >= 0 ? 4 * (pacf_want + 1) : 0));
+    B.nscr = even(std::max(64, (basic_bins + 1) / 2));      // launch_basic raises it to the series length
+    for (int q = 0, prev = -1; q < (int)P->host[G_BASIC].size(); ++q) {       // distinct agg_linear_trend keys
+        const Desc& d = P->host[G_BASIC][q];
+        const int key = (d.i0 << 4) | d.i1;
+        if (d.calc == TSFX_AGG_LINEAR_TREND && key != prev) { ++B.nalt; prev = key; }
+    }
+    B.dec = ctx->d_dec;
+    SortedArgs& S = P->sorted;
+    group(S, G_SORTED);
+    S.nscr = even(4 * (friedrich_r + 2) + 16);
+    S.nfin = sorted_nfin;
+    double pl = -1.0, ph = -1.0;                                 // distinct change_quantiles corridors
+    for (const Desc& d : P->host[G_SORTED])
+        if (d.calc == TSFX_CHANGE_QUANTILES && !(d.p0 == pl && d.p1 == ph)) { ++S.ncq; pl = d.p0; ph = d.p1; }
+    SpectralArgs& F = P->spectral;
+    group(F, G_SPECTRAL);
+    F.tables = P->d_tables; F.table_off = P->d_toff; F.table_half = P->d_thalf;
+    F.need_fft = need_fft; F.need_welch = need_welch;
+    F.max_hist = fourier_bins;
+    F.nfft = spectral_nfft;
+    group(P->la, G_LA);
+    P->la.max_ar_k = max_ar_k;
+    group(P->entropy, G_ENTROPY);
+    SeqArgs& Q = P->seq;
+    group(Q, G_SEQ);
+    Q.need_lz = max_lz_bins > 0; Q.need_perm = max_perm_dim > 0;
+    Q.n_lz = n_lz; Q.max_lz_bins = max_lz_bins;
+    group(P->peaks, G_PEAKS);
+    P->peaks.cwt_n = max_cwt_peaks_n;
     *out = P;
     return TSFX_OK;
 }
@@ -572,7 +616,6 @@ extern "C" void tsfx_plan_destroy(tsfx_plan* P) {
 }
 
 // ------------------------------------------------------------------------------------------ launch all groups
-static int even(int v) { return (v + 1) & ~1; }
 
 static int ensure_twiddle(tsfx_ctx* ctx, int n_pow2) {
     if (n_pow2 <= ctx->tw_n) return TSFX_OK;
@@ -630,8 +673,6 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
     if (staged == 0) return TSFX_OK;
     CK(ctx->stage.reserve((size_t)R.n_series * staged * sizeof(double)));
     CK(ctx->misc.reserve(max_len > 1024 ? ((size_t)1 << 30) : ((size_t)256 << 20)));      // global working regions for series too long for shared memory
-    double* const d_final = d_out;
-    (void)d_final;
     if (!P->host[G_SPECTRAL].empty()) {      // FFT twiddle table (filled once, on the main stream, before any fork)
         int p2 = 1;
         while (p2 < max_len) p2 <<= 1;
@@ -663,7 +704,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         if (timing) { CK(cudaEventRecord(ctx->ev[g][0], ctx->stream)); }
         cudaError_t e = cudaSuccess;
         const char* variant = nullptr;
-        double* d_out = (double*)ctx->stage.p + (size_t)R.n_series * P->cum[g];      // this group's staging matrix
+        double* const stage_g = (double*)ctx->stage.p + (size_t)R.n_series * P->cum[g];      // this group's staging matrix
         const int sidx = launched++ % nstreams;
         cudaStream_t gs = (sidx == 0) ? ctx->stream : ctx->s_side[sidx - 1];
         const int g_ncols = (int)P->host[g].size();
@@ -671,6 +712,11 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         // they overlap on side streams (concurrent groups must not share working sets)
         const size_t slice = (nstreams > 1) ? (ctx->misc.cap / G_COUNT) & ~(size_t)255 : ctx->misc.cap;
         unsigned char* const gs_base = (unsigned char*)ctx->misc.p + (nstreams > 1 ? (size_t)g * slice : 0);
+        // the plan's arguments of the group with this call's series, working region and staging matrix
+        auto call = [&](auto A) {
+            A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.out = stage_g;
+            return A;
+        };
         switch (g) {
             case G_BASIC: {
                 if (P->basic_moments_only) {
@@ -679,91 +725,37 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                     MomentsArgs M;
                     M.R = R; M.descs = P->dev[g]; M.nd = g_ncols; M.need_high = P->moments_need_high;
                     direct = (P->n_groups_used == 1) && ctx->peer_out.empty() && (P->ncols == g_ncols);
-                    M.out = direct ? d_final : d_out;
+                    M.out = direct ? d_out : stage_g;
                     M.ncols = direct ? ld : g_ncols;
                     M.colmap = direct ? P->d_final_col + P->cum[g] : nullptr;
                     e = launch_moments(M, gs, ctx->sm_count, &variant);
                     ctx->used_moments = true;
                     break;
                 }
-                BasicArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                A.lag_needed = P->lag_needed;
-                A.nfin = P->basic_nfin;
-                int pac = P->pacf_want >= 0 ? 4 * (P->pacf_want + 1) : 0;
-                A.pacf_off = P->lag_needed + 1;
-                A.nlag = even(P->lag_needed + 1 + pac);
-                A.nscr = even(std::max(std::max(max_len, 64), (P->basic_bins + 1) / 2));
-                A.nalt = 0;
-                {
-                    int prev = -1;
-                    for (const Desc& q : P->host[g])
-                        if (q.calc == TSFX_AGG_LINEAR_TREND) {
-                            const int key = (q.i0 << 4) | q.i1;
-                            if (key != prev) { ++A.nalt; prev = key; }
-                        }
-                }
-                A.dec = ctx->d_dec;
-                e = launch_basic(A, max_len, gs, ctx->sm_count, &variant);
+                e = launch_basic(call(P->basic), max_len, gs, ctx->sm_count, &variant);
                 break;
             }
-            case G_SORTED: {
-                SortedArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                A.nscr = even(4 * (P->friedrich_r + 2) + 16);
-                A.nfin = P->sorted_nfin;
-                A.ncq = 0;
-                {
-                    double pl = -1.0, ph = -1.0;
-                    for (const Desc& q : P->host[g])
-                        if (q.calc == TSFX_CHANGE_QUANTILES && !(q.p0 == pl && q.p1 == ph)) { ++A.ncq; pl = q.p0; ph = q.p1; }
-                }
-                e = launch_sorted(A, max_len, gs, ctx->sm_count, &variant);
-                break;
-            }
+            case G_SORTED: e = launch_sorted(call(P->sorted), max_len, gs, ctx->sm_count, &variant); break;
             case G_SPECTRAL: {
-                SpectralArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
+                SpectralArgs A = call(P->spectral);
                 A.twiddle = ctx->d_tw; A.tw_n = ctx->tw_n;
-                A.tables = P->d_tables; A.table_off = P->d_toff; A.table_half = P->d_thalf;
-                A.need_fft = P->need_fft; A.need_welch = P->need_welch;
-                A.max_hist = P->fourier_bins;
-                A.nfft = P->spectral_nfft;
                 e = launch_spectral(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
-            case G_LA: {
-                LaArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                A.nscr = P->max_ar_k;
-                e = launch_la(A, max_len, gs, ctx->sm_count, &variant);
-                break;
-            }
-            case G_ENTROPY: {
-                EntropyArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                e = launch_entropy(A, max_len, gs, ctx->sm_count, &variant);
-                break;
-            }
-            case G_SEQ: {
-                SeqArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                A.nscr = (P->max_lz_bins > 0 ? 1 : 0) | (P->max_perm_dim > 0 ? 2 : 0) | (P->max_cwt_peaks_n << 8) |
-                         (std::min(P->n_lz, 255) << 16) | (std::min(P->max_lz_bins, 255) << 24);
-                e = launch_seq(A, max_len, gs, ctx->sm_count, &variant);
-                break;
-            }
+            case G_LA: e = launch_la(call(P->la), max_len, gs, ctx->sm_count, &variant); break;
+            case G_ENTROPY: e = launch_entropy(call(P->entropy), max_len, gs, ctx->sm_count, &variant); break;
+            case G_SEQ: e = launch_seq(call(P->seq), max_len, gs, ctx->sm_count, &variant); break;
             case G_PEAKS: {
-                SeqArgs A;
-                A.R = R; A.gscratch = gs_base; A.gscratch_bytes = slice; A.descs = P->dev[g]; A.nd = (int)P->host[g].size(); A.out = d_out; A.ncols = g_ncols;
-                A.nscr = (P->max_cwt_peaks_n << 8);
+                PeaksArgs A = call(P->peaks);
                 A.ricker = ctx->d_ricker;
                 e = launch_peaks(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
         }
         if (e == cudaErrorInvalidConfiguration) return too_long(kGroupNames[g]);
-        if (e != cudaSuccess) return fail(ctx, TSFX_E_CUDA, std::string("launch ") + kGroupNames[g] + ": " + cudaGetErrorString(e));
+        if (e != cudaSuccess)      // the variant names the geometry of a launch that failed, or one not compiled
+            return fail(ctx, TSFX_E_CUDA, std::string("launch ") + kGroupNames[g] + (variant ? std::string(" (") + variant + ")" : "") +
+                                              ": " + cudaGetErrorString(e));
         ctx->launches += 1;
         ctx->kernels[ctx->n_kernels++] = variant;
         if (timing) { CK(cudaEventRecord(ctx->ev[g][1], ctx->stream)); ctx->ev_used[g] = true; }
@@ -776,7 +768,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
     if (!direct) {   // scatter the staging matrices into the caller's [n_series x ncols] matrix
         if (timing) { CK(cudaEventRecord(ctx->ev[G_COUNT][0], ctx->stream)); }
         AssembleArgs A;
-        A.stage = (const double*)ctx->stage.p; A.out = d_final; A.n_series = R.n_series; A.ncols = P->ncols; A.ld = ld;
+        A.stage = (const double*)ctx->stage.p; A.out = d_out; A.n_series = R.n_series; A.ncols = P->ncols; A.ld = ld;
         if (ld != P->ncols && !ctx->peer_out.empty()) return fail(ctx, TSFX_E_UNSUPPORTED, "peer placement of a strided matrix");
         A.n_groups = G_COUNT;
         for (int g = 0; g <= G_COUNT; ++g) A.cum[g] = P->cum[g];
@@ -784,11 +776,11 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         A.n_extra = 0;
         A.out_mc = nullptr;
         // multi-GPU placement: where does this row block live inside the peers' copies of the result matrix?
-        int64_t peer_off = -1;                 // byte offset of d_final inside this rank's mapped matrix
+        int64_t peer_off = -1;                 // byte offset of d_out inside this rank's mapped matrix
         if (!ctx->peer_out.empty()) {
             const uint64_t self = ctx->peer_out[ctx->peer_self];
-            if ((uint64_t)d_final < self) return fail(ctx, TSFX_E_INVALID, "out is not inside the matrix registered with tsfx_set_peer_outputs");
-            peer_off = (int64_t)((uint64_t)d_final - self);
+            if ((uint64_t)d_out < self) return fail(ctx, TSFX_E_INVALID, "out is not inside the matrix registered with tsfx_set_peer_outputs");
+            peer_off = (int64_t)((uint64_t)d_out - self);
             if (ctx->peer_mode == TSFX_PEER_MULTICAST) A.out_mc = (double*)(ctx->peer_mc + (uint64_t)peer_off);
             else if (ctx->peer_mode == TSFX_PEER_STORE)
                 for (size_t p = 0; p < ctx->peer_out.size(); ++p)
@@ -806,7 +798,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
             const size_t np = ctx->peer_out.size();
             for (size_t k = 1; k < np; ++k) {          // start with the next rank so the ranks do not all hit one peer
                 const size_t p = ((size_t)ctx->peer_self + k) % np;
-                CK(cudaMemcpyAsync((void*)(ctx->peer_out[p] + (uint64_t)peer_off), d_final, bytes, cudaMemcpyDeviceToDevice, ctx->s_peer));
+                CK(cudaMemcpyAsync((void*)(ctx->peer_out[p] + (uint64_t)peer_off), d_out, bytes, cudaMemcpyDeviceToDevice, ctx->s_peer));
             }
         }
     }
@@ -1009,19 +1001,17 @@ extern "C" int tsfx_last_kernels(const tsfx_ctx* ctx, const char** names_out, in
     return k;
 }
 
-// every name a launcher can report (TSFX_GEOM_NAMES expands to the six plan_geometry placements of a kernel)
-#define TSFX_GEOM_LIST(GRP) GRP "/w8/shared", GRP "/w4/shared", GRP "/w2/shared", GRP "/w1/shared", GRP "/w4/global", GRP "/w1/global"
+// every name a launcher can report: its fixed-geometry kernels and its declared geometries (tsfx_kernels.h)
 static const char* const kKernelVariants[] = {
     "moments/dense", "moments/general",
-    "basic/w12/shared", "basic/w24/shared", TSFX_GEOM_LIST("basic"),
-    "sorted/w12/shared", TSFX_GEOM_LIST("sorted"),
-    TSFX_GEOM_LIST("spectral"), TSFX_GEOM_LIST("spectral/pow2"),
-    "la/small", TSFX_GEOM_LIST("la"),
-    "entropy/rank-g1", "entropy/rank-g4", "entropy/rank-g16", TSFX_GEOM_LIST("entropy/tiles"), TSFX_GEOM_LIST("entropy/pairs"),
-    "seq/small", TSFX_GEOM_LIST("seq/general"),
-    "peaks/small", TSFX_GEOM_LIST("peaks/general"), "peaks/general/hybrid/w4/global", "peaks/general/hybrid/w1/global",
+    TSFX_GEOMS_BASIC(TSFX_GEOM_NAME, "basic")
+    TSFX_GEOMS_ALL(TSFX_GEOM_NAME, "sorted")
+    TSFX_GEOMS_ALL(TSFX_GEOM_NAME, "spectral") TSFX_GEOMS_ALL(TSFX_GEOM_NAME, "spectral/pow2")
+    "la/small", TSFX_GEOMS_ALL(TSFX_GEOM_NAME, "la")
+    "entropy/rank-g1", "entropy/rank-g4", "entropy/rank-g16", TSFX_GEOMS_ENTROPY(TSFX_GEOM_NAME, "entropy/tiles")
+    "seq/small", TSFX_GEOMS_SEQ(TSFX_GEOM_NAME, "seq/general")
+    "peaks/small", TSFX_GEOMS_PEAKS(TSFX_GEOM_NAME, "peaks/general") TSFX_GEOMS_PEAKS(TSFX_GEOM_NAME, "peaks/general/hybrid")
 };
-#undef TSFX_GEOM_LIST
 
 extern "C" int tsfx_kernel_variants(const char** names_out, int32_t cap) {
     const int n = (int)(sizeof(kKernelVariants) / sizeof(kKernelVariants[0]));
