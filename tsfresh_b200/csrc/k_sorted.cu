@@ -12,6 +12,13 @@
 #include "tsfx_kernels.h"
 #include "tsfx_math.cuh"
 
+// Builds for profiles/scripts/time_sorted_phases.py: -DTSFX_SORTED_SKIP=k leaves phase k out (1 the sort, 2 the
+// finishers, 3 change_quantiles, 4 the Friedrich fit, 5 mean_n_absolute_max), so the group's time splits by phase.
+// Their results are wrong; the library build never sets it.
+#ifndef TSFX_SORTED_SKIP
+#define TSFX_SORTED_SKIP 0
+#endif
+
 namespace tsfx {
 
 __device__ __forceinline__ void warp_bitonic_sort(float* s, int m, int lane) {
@@ -27,6 +34,26 @@ __device__ __forceinline__ void warp_bitonic_sort(float* s, int m, int lane) {
             __syncwarp();
         }
     }
+}
+
+// change_quantiles corridors served by one sweep over the pairs: pass 2 holds 4 doubles and 2 floats per corridor in
+// registers, and with four the pair loops of the 8-warp kernel (at most 80 registers) stay free of spills
+#define CQ_BATCH 4
+
+// Sums v[0..7] over the warp in the butterfly order of wsum (xor offsets 16, 8, 4, 2, 1), so sum k is bit-identical to
+// wsum(v[k]); it ends in lanes 4k .. 4k+3.  The first three steps each hand half of the remaining sums to the partner
+// lane: 9 double shuffles instead of 40.
+__device__ __forceinline__ double wsum8_scatter(const double (&v)[8], int lane) {
+    const bool u16 = lane & 16, u8 = lane & 8, u4 = lane & 4;
+    double a[4], b[2];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) a[k] = (u16 ? v[k + 4] : v[k]) + __shfl_xor_sync(FULL, u16 ? v[k] : v[k + 4], 16);
+#pragma unroll
+    for (int k = 0; k < 2; ++k) b[k] = (u8 ? a[k + 2] : a[k]) + __shfl_xor_sync(FULL, u8 ? a[k] : a[k + 2], 8);
+    double c = (u4 ? b[1] : b[0]) + __shfl_xor_sync(FULL, u4 ? b[0] : b[1], 4);
+    c += __shfl_xor_sync(FULL, c, 2);
+    c += __shfl_xor_sync(FULL, c, 1);
+    return c;
 }
 
 struct Uniq { int n_unique, n_reocc_values, n_reocc_points; double sum_reocc_values, sum_reocc_points; bool any_dup; };
@@ -233,7 +260,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
         }
         sum = wsum(sum);
         __syncwarp();
-        warp_bitonic_sort(srt, m, lane);
+        if (TSFX_SORTED_SKIP != 1) warp_bitonic_sort(srt, m, lane);
         const double dn = (double)n;
         const double mean = sum / dn;
         const double vmin = (double)srt[0], vmax = (double)srt[n - 1];
@@ -246,7 +273,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
 
         // O(1) "finishers" (the first A.nfin descriptors): order statistics and the unique-value counts, one
         // descriptor per lane
-        if (A.nfin > 0) {
+        if (A.nfin > 0 && TSFX_SORTED_SKIP != 2) {
             const Uniq U = unique_pass(srt, n, lane);
             if (live)
                 for (int j = lane; j < A.nfin; j += 32) {
@@ -288,7 +315,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
             switch (d.calc) {
                 case TSFX_MEAN_N_ABSOLUTE_MAX: {
                     int k = d.i0;
-                    if (n <= k) { r = dnan(); break; }
+                    if (n <= k || TSFX_SORTED_SKIP == 5) { r = dnan(); break; }
                     double acc = 0.0;
                     if (lane == 0) {
                         int a = 0, b = n - 1;
@@ -302,49 +329,91 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                 }
                 case TSFX_CHANGE_QUANTILES: {
                     // stage A, warp-uniform: every distinct corridor (ql, qh) of the run -> count, mean and variance of
-                    // the changes and of their magnitudes (two passes serve all four (isabs, f_agg) columns);
-                    // stage B: one descriptor per lane picks its column
+                    // the changes and of their magnitudes (two passes serve all four (isabs, f_agg) columns), CQ_BATCH
+                    // corridors per sweep over the pairs; stage B: one descriptor per lane picks its column
                     used = run;
                     stored = true;
-                    int slot = 0;
-                    double pl = -1.0, ph = -1.0;
-                    for (int t = 0; t < run; ++t) {
-                        const double ql = A.descs[j + t].p0, qh = A.descs[j + t].p1;
-                        if (ql == pl && qh == ph) continue;
-                        pl = ql; ph = qh;
-                        int cnt = 0;
-                        double mean0 = 0.0, mean1 = 0.0, var0 = 0.0, var1 = 0.0;
-                        if (ql < qh) {
-                            const double lo = m_quantile_sorted(srt, n, ql), hi = m_quantile_sorted(srt, n, qh);
-                            int c = 0;
-                            double s1 = 0.0, s1a = 0.0;
-                            for (int i = lane; i + 1 < n; i += 32) {
-                                const double a = (double)xs[i], b = (double)xs[i + 1];
-                                if (a >= lo && a <= hi && b >= lo && b <= hi) { const double dx = b - a; s1 += dx; s1a += fabs(dx); ++c; }
-                            }
-                            cnt = wsumi(c);
-                            mean0 = wsum(s1) / (double)cnt;
-                            mean1 = wsum(s1a) / (double)cnt;
-                            double q2 = 0.0, q2a = 0.0;
-                            if (cnt > 0)
-                                for (int i = lane; i + 1 < n; i += 32) {
-                                    const double a = (double)xs[i], b = (double)xs[i + 1];
-                                    if (a >= lo && a <= hi && b >= lo && b <= hi) {
-                                        const double dx = b - a, e = dx - mean0, ea = fabs(dx) - mean1;
-                                        q2 = fma(e, e, q2);
-                                        q2a = fma(ea, ea, q2a);
-                                    }
+                    if (TSFX_SORTED_SKIP == 3) break;
+                    for (int c0 = 0; c0 < A.ncq; c0 += CQ_BATCH) {
+                        // bounds of the batch, one per lane (lane 2k: lower bound of corridor c0 + k, lane 2k + 1: upper),
+                        // as float32 thresholds: for every float x, including +-inf and NaN, x >= Q <=> x >= ru(Q) and
+                        // x <= Q <=> x <= rd(Q).  Corridors with ql >= qh, and slots past the last corridor, get NaN,
+                        // which no sample meets: their count is 0.
+                        float th = __int_as_float(0x7fffffff);
+                        if (lane < 2 * CQ_BATCH && c0 + (lane >> 1) < A.ncq) {
+                            const double2 q = A.cq[c0 + (lane >> 1)];
+                            if (q.x < q.y)
+                                th = (lane & 1) ? __double2float_rd(m_quantile_sorted(srt, n, q.y))
+                                                : __double2float_ru(m_quantile_sorted(srt, n, q.x));
+                        }
+                        float lo[CQ_BATCH], hi[CQ_BATCH];
+#pragma unroll
+                        for (int k = 0; k < CQ_BATCH; ++k) {
+                            lo[k] = __shfl_sync(FULL, th, 2 * k);
+                            hi[k] = __shfl_sync(FULL, th, 2 * k + 1);
+                        }
+                        // pass 1: v[k] = sum of the changes inside corridor c0 + k, v[CQ_BATCH + k] = of their magnitudes
+                        int c[CQ_BATCH];
+                        double v[2 * CQ_BATCH];
+#pragma unroll
+                        for (int k = 0; k < CQ_BATCH; ++k) { c[k] = 0; v[k] = 0.0; v[CQ_BATCH + k] = 0.0; }
+                        for (int i = lane; i + 1 < n; i += 32) {
+                            const float a = xs[i], b = xs[i + 1];
+                            const double dx = (double)b - (double)a;
+#pragma unroll
+                            for (int k = 0; k < CQ_BATCH; ++k)
+                                if (a >= lo[k] && a <= hi[k] && b >= lo[k] && b <= hi[k]) {
+                                    v[k] += dx;
+                                    v[CQ_BATCH + k] += fabs(dx);
+                                    ++c[k];
                                 }
-                            var0 = wsum(q2) / (double)cnt;
-                            var1 = wsum(q2a) / (double)cnt;
                         }
-                        if (lane == 0 && slot < A.ncq) {
-                            double* S = cqS + 5 * slot;
-                            S[0] = (double)cnt; S[1] = mean0; S[2] = mean1; S[3] = var0; S[4] = var1;
+                        // lane L ends with sum L / 4: corridor (L / 4) % CQ_BATCH, changes in lanes 0-15, magnitudes in 16-31
+                        const int me = (lane >> 2) & (CQ_BATCH - 1);
+                        const int slot = c0 + me;
+                        const bool writer = (lane & 3) == 0 && slot < A.ncq;
+                        int cnt = 0;
+                        bool any = false;
+#pragma unroll
+                        for (int k = 0; k < CQ_BATCH; ++k) {
+                            const int ck = wsumi(c[k]);
+                            any |= ck > 0;
+                            if (k == me) cnt = ck;
                         }
-                        ++slot;
+                        double* S = cqS + 5 * slot;
+                        const double mean = wsum8_scatter(v, lane) / (double)cnt;
+                        if (writer) {
+                            if (lane < 16) S[0] = (double)cnt;
+                            S[1 + (lane >> 4)] = mean;
+                        }
+                        __syncwarp();
+                        if (any) {
+                            // pass 2: squared deviations from the corridor's means, same order as pass 1
+                            double m0[CQ_BATCH], m1[CQ_BATCH], q[2 * CQ_BATCH];
+#pragma unroll
+                            for (int k = 0; k < CQ_BATCH; ++k) {
+                                const bool ok = c0 + k < A.ncq;
+                                m0[k] = ok ? cqS[5 * (c0 + k) + 1] : 0.0;
+                                m1[k] = ok ? cqS[5 * (c0 + k) + 2] : 0.0;
+                                q[k] = 0.0;
+                                q[CQ_BATCH + k] = 0.0;
+                            }
+                            for (int i = lane; i + 1 < n; i += 32) {
+                                const float a = xs[i], b = xs[i + 1];
+                                const double dx = (double)b - (double)a;
+#pragma unroll
+                                for (int k = 0; k < CQ_BATCH; ++k)
+                                    if (a >= lo[k] && a <= hi[k] && b >= lo[k] && b <= hi[k]) {
+                                        const double e = dx - m0[k], ea = fabs(dx) - m1[k];
+                                        q[k] = fma(e, e, q[k]);
+                                        q[CQ_BATCH + k] = fma(ea, ea, q[CQ_BATCH + k]);
+                                    }
+                            }
+                            const double var = wsum8_scatter(q, lane) / (double)cnt;
+                            if (writer) S[3 + (lane >> 4)] = var;
+                        }
+                        __syncwarp();
                     }
-                    __syncwarp();
                     int base_slot = -1;
                     double last_l = -1.0, last_h = -1.0;
                     for (int t0 = 0; t0 < run; t0 += 32) {
@@ -373,6 +442,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                 }
                 case TSFX_FRIEDRICH_COEFFICIENTS:
                 case TSFX_MAX_LANGEVIN_FIXED_POINT: {
+                    if (TSFX_SORTED_SKIP == 4) { r = dnan(); break; }
                     if (fr_r != d.i2) {
                         __syncwarp();
                         fr_ok = friedrich_fit(xs, srt, n, d.i2, scr, coef, lane);

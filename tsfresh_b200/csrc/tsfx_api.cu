@@ -277,6 +277,7 @@ struct tsfx_plan {
     std::vector<Desc> host[G_COUNT];
     Desc* dev[G_COUNT] = {nullptr};
     int32_t* d_final_col = nullptr;   // final column of every staged column, groups concatenated
+    double2* d_cq = nullptr;          // (ql, qh) of the distinct change_quantiles corridors (SortedArgs::cq)
     bool basic_moments_only = false;  // the BASIC group is reductions only: k_moments replaces k_basic
     int moments_need_high = 0;
     int n_groups_used = 0;
@@ -583,8 +584,16 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
     S.nscr = even(4 * (friedrich_r + 2) + 16);
     S.nfin = sorted_nfin;
     double pl = -1.0, ph = -1.0;                                 // distinct change_quantiles corridors
+    std::vector<double2> cq;
     for (const Desc& d : P->host[G_SORTED])
-        if (d.calc == TSFX_CHANGE_QUANTILES && !(d.p0 == pl && d.p1 == ph)) { ++S.ncq; pl = d.p0; ph = d.p1; }
+        if (d.calc == TSFX_CHANGE_QUANTILES && !(d.p0 == pl && d.p1 == ph)) { cq.push_back(make_double2(d.p0, d.p1)); pl = d.p0; ph = d.p1; }
+    S.ncq = (int)cq.size();
+    if (!cq.empty()) {
+        cudaError_t e = cudaMalloc(&P->d_cq, cq.size() * sizeof(double2));
+        if (e == cudaSuccess) e = cudaMemcpy(P->d_cq, cq.data(), cq.size() * sizeof(double2), cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { tsfx_plan_destroy(P); return fail(ctx, TSFX_E_CUDA, cudaGetErrorString(e)); }
+    }
+    S.cq = P->d_cq;
     SpectralArgs& F = P->spectral;
     group(F, G_SPECTRAL);
     F.tables = P->d_tables; F.table_off = P->d_toff; F.table_half = P->d_thalf;
@@ -609,6 +618,7 @@ extern "C" void tsfx_plan_destroy(tsfx_plan* P) {
     if (P->ctx) cudaSetDevice(P->ctx->device);
     for (int g = 0; g < G_COUNT; ++g) if (P->dev[g]) cudaFree(P->dev[g]);
     if (P->d_final_col) cudaFree(P->d_final_col);
+    if (P->d_cq) cudaFree(P->d_cq);
     if (P->d_tables) cudaFree(P->d_tables);
     if (P->d_toff) cudaFree(P->d_toff);
     if (P->d_thalf) cudaFree(P->d_thalf);

@@ -196,6 +196,7 @@ bool moments_only_calc(int calc);       // host: can the reduction-only kernel e
 struct SortedArgs : GroupArgs {
     int npad, npow2, nscr, bytes_per_warp;
     int nfin, ncq;       // leading O(1) descriptors (lane-parallel); distinct change_quantiles corridors
+    const double2* cq;   // device: (ql, qh) of every distinct corridor, in descriptor order
 };
 cudaError_t launch_sorted(const SortedArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
