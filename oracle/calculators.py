@@ -279,14 +279,21 @@ def change_quantiles(x, ql, qh, isabs, f_agg):  # :1511-1553
     return getattr(np, f_agg)(d[np.where(both == 1)])
 
 
-def _friedrich_fit(x, m, r):  # :131-173
+def friedrich_points(x, r):  # :131-170
+    """the (signal mean, delta mean) of every non-empty quantile bin, or None where pd.qcut fails"""
     frame = pd.DataFrame({"signal": x[:-1], "delta": np.diff(x)})
     try:
         frame["q"] = pd.qcut(frame.signal, r)
     except (ValueError, IndexError):
-        return [NAN] * (m + 1)
+        return None
     g = frame.groupby("q", observed=False)
-    pts = pd.DataFrame({"xm": g.signal.mean(), "ym": g.delta.mean()}).dropna()
+    return pd.DataFrame({"xm": g.signal.mean(), "ym": g.delta.mean()}).dropna()
+
+
+def _friedrich_fit(x, m, r):  # :131-173
+    pts = friedrich_points(x, r)
+    if pts is None:
+        return [NAN] * (m + 1)
     try:
         return np.polyfit(pts.xm, pts.ym, deg=m)
     except (np.linalg.LinAlgError, ValueError):

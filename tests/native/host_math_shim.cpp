@@ -7,7 +7,7 @@ double hm_incbeta(double a, double b, double x) { return m_incbeta(a, b, x); }
 double hm_student2(double t, double df) { return m_student_two_sided(t, df); }
 double hm_mackinnon(double s) { return m_mackinnon_p_c(s); }
 double hm_cubic(double a, double b, double c, double d) { return m_poly3_max_real_root(a, b, c, d); }
-int hm_polyfit3(const double* x, const double* y, int k, double* c) { return m_polyfit3(x, y, k, c) ? 1 : 0; }
+int hm_polyfit3(const double* x, const double* y, int k, double* c /*5*/) { return m_polyfit3(x, y, k, c) ? 1 : 0; }
 void hm_levinson(const double* acv, int nlags, double* out, double* work) { m_levinson_pacf(acv, nlags, out, work); }
 double hm_quantile(const double* s, int n, double q) { return m_quantile_sorted(s, n, q); }
 void hm_linreg(double n, double xm, double ym, double sxx, double syy, double sxy, double* o) {

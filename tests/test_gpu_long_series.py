@@ -95,13 +95,13 @@ def want():
     """oracle rows of every series of the module (one pool pass, longest series first, each array once)"""
     import multiprocessing as mp
 
-    from tests.test_gpu_shapes import _cores
+    from tests.helpers import cores
     groups = [(name, c[0]) for name, c in CASES.items()] + [("frame", FRAME), ("roll", ROLL_WINDOWS)]
     unique = {}
     for _, ss in groups:
         for s in ss:
             unique.setdefault(id(s), s)
-    with mp.get_context("spawn").Pool(_cores()) as pool:
+    with mp.get_context("spawn").Pool(cores()) as pool:
         rows = dict(zip(unique, oracle(pool, EfficientFCParameters(), list(unique.values()))))
     return {name: np.asarray([rows[id(s)] for s in ss]) for name, ss in groups}
 

@@ -17,7 +17,7 @@ import numpy as np
 import pytest
 
 from oracle.extract import compare, oracle_rows
-from tests.helpers import synthetic_series, to_csr
+from tests.helpers import cores, synthetic_series, to_csr
 from tsfresh_b200.plan import Plan
 from tsfresh_b200.settings import ComprehensiveFCParameters, EfficientFCParameters
 
@@ -32,22 +32,11 @@ def _oracle_chunk(args):
     return oracle_rows([np.asarray(s, dtype=np.float32).astype(np.float64) for s in chunk], SETTINGS[name]())
 
 
-def _cores():
-    n = len(os.sched_getaffinity(0))
-    try:
-        quota, period = open("/sys/fs/cgroup/cpu.max").read().split()
-        if quota != "max":
-            n = min(n, max(1, int(round(int(quota) / int(period)))))
-    except Exception:
-        pass
-    return max(1, n)
-
-
 def oracle_parallel(series, name):
-    cores = _cores()
-    per = max(1, (len(series) + 4 * cores - 1) // (4 * cores))
+    n = cores()
+    per = max(1, (len(series) + 4 * n - 1) // (4 * n))
     chunks = [(name, series[i:i + per]) for i in range(0, len(series), per)]
-    with mp.get_context("spawn").Pool(cores) as pool:
+    with mp.get_context("spawn").Pool(n) as pool:
         parts = pool.map(_oracle_chunk, chunks)
     return np.concatenate(parts, axis=0)
 

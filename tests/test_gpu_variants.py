@@ -27,8 +27,7 @@ import numpy as np
 import pytest
 
 from oracle.extract import NOISE_FLOOR, compare, oracle_rows
-from tests.helpers import to_csr
-from tests.test_gpu_shapes import _cores
+from tests.helpers import cores, to_csr
 from tsfresh_b200.plan import Plan
 from tsfresh_b200.settings import ComprehensiveFCParameters, MinimalFCParameters
 
@@ -109,7 +108,7 @@ def ctx():
 
 @pytest.fixture(scope="module")
 def pool():
-    with mp.get_context("spawn").Pool(_cores()) as p:
+    with mp.get_context("spawn").Pool(cores()) as p:
         yield p
 
 

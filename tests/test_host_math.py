@@ -3,6 +3,7 @@ the host with g++ and checked against scipy / numpy.  CPU-only."""
 import ctypes
 import os
 import subprocess
+import warnings
 
 import numpy as np
 import pytest
@@ -59,13 +60,59 @@ def test_polyfit3(hm):
     for k in (1, 2, 3, 4, 5, 12, 30):
         x = np.sort(rng.standard_normal(k) * 2)
         y = rng.standard_normal(k)
-        c = np.zeros(4)
+        c = np.zeros(5)
         assert hm.hm_polyfit3(_p(x), _p(y), k, _p(c))
-        import warnings
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
             want = np.polyfit(x, y, 3)
-        np.testing.assert_allclose(c, want, rtol=1e-7, atol=1e-9)
+        np.testing.assert_allclose(c[:4], want, rtol=1e-7, atol=1e-9)
+
+
+def _shifted_fits():
+    """(level, r, bin means x, y) of the Friedrich fit (the oracle's bin means) on walks b + 0.3 cumsum(N(0, 1)) of 256
+    float32 samples, and on 31-sample N(0, 1) series for k = 1 .. 3 bins"""
+    from oracle.calculators import friedrich_points
+    rng = np.random.default_rng(11)
+    out = []
+    for level in (0.0, 30.0, 100.0, 300.0, 1e3, 3e3, 1e4, -1e3):
+        for i in range(6):
+            walk = (level + 0.3 * rng.standard_normal(256).cumsum()).astype(np.float32).astype(np.float64)
+            short = (level + rng.standard_normal(31)).astype(np.float32).astype(np.float64)
+            for s, r in ((walk, 4), (walk, 5), (walk, 10), (walk, 30), (short, 1), (short, 2), (short, 3)):
+                pts = friedrich_points(s, r)
+                out.append((level, r, pts.xm.to_numpy(np.float64), pts.ym.to_numpy(np.float64)))
+    return out
+
+
+def test_polyfit3_shifted_abscissae(hm):
+    """Bin means at levels up to 1e4: the coefficients against the exact least-squares (k >= 4) or minimum-norm (k < 4)
+    fit within the least-squares perturbation bound (tests/helpers.py:polyfit3_accepts), against np.polyfit at
+    rtol 1e-5 where that bound is below 1e-7, and the largest real root against np.roots of the exact fit"""
+    from oracle.extract import NOISE_FLOOR
+    from tests.helpers import exact_polyfit3, polyfit3_bound, polyfit3_error
+    failures = []
+    for level, r, x, y in _shifted_fits():
+        k = len(x)
+        c = np.zeros(5)
+        if not hm.hm_polyfit3(_p(x), _p(y), k, _p(c)):
+            failures.append((level, r, k, "no fit"))
+            continue
+        ex, S = exact_polyfit3(x, y)
+        err, bound = polyfit3_error(c[:4], ex, S), polyfit3_bound(x, y, ex, S)
+        if not err <= max(1e-5, bound):
+            failures.append((level, r, k, "coefficients", err, bound))
+        if bound < 1e-7:
+            with warnings.catch_warnings():
+                warnings.simplefilter("ignore")
+                want = np.polyfit(x, y, 3)
+            if not np.allclose(c[:4], want, rtol=1e-5, atol=0):
+                failures.append((level, r, k, "np.polyfit", list(c[:4]), list(want)))
+        # the roots live at the scale of the abscissae: one bin gives the cubic c (t^3 + t^2 x + t x^2 + x^3) with the
+        # roots -x and +-ix, so a largest real part of exactly 0 that both sides compute as rounding noise of order eps |x|
+        root = np.max(np.real(np.roots([float(v) for v in ex])))
+        if not np.isclose(c[4], root, rtol=1e-5, atol=NOISE_FLOOR * max(1.0, np.abs(x).max())):
+            failures.append((level, r, k, "max_langevin", c[4], root))
+    assert not failures, "%d failures, first: %r" % (len(failures), failures[:10])
 
 
 def test_levinson_quantile_linreg_cholesky(hm):

@@ -102,13 +102,18 @@ __device__ __forceinline__ double quantile_view(const DropLast& v, int n, double
 }
 
 // np.polyfit(x, y, 3) for k >= 4 points held in shared memory, all lanes cooperating (points strided over
-// lanes): column-scaled normal equations, 4x4 Cholesky done redundantly by every lane, two refinement steps
-// with residuals formed from the data (same algebra as m_polyfit3, which stays for the k < 4 minimum-norm case).
+// lanes): the k >= 4 algebra of m_polyfit3 (centred variable, column-scaled normal equations, two refinement steps with
+// residuals formed from the data) with lane-parallel sums; the 4x4 Cholesky is done redundantly by every lane.
+// coef[0..3] = coefficients, coef[4] = max_langevin_fixed_point.
 __device__ __forceinline__ bool warp_polyfit3(const double* x, const double* y, int k, double* coef, int lane) {
+    // the bin means come in bin order, so the first and the last span the points' range
+    double mu, h;
+    if (!m_cubic_centre(fmin(x[0], x[k - 1]), fmax(x[0], x[k - 1]), &mu, &h)) return false;
+    const double ih = 1.0 / h;
     double sc[4] = {0, 0, 0, 0};
     for (int i = lane; i < k; i += 32) {
-        const double v = x[i], v2 = v * v, v3 = v2 * v;
-        sc[0] = fma(v3, v3, sc[0]); sc[1] = fma(v2, v2, sc[1]); sc[2] = fma(v, v, sc[2]); sc[3] += 1.0;
+        const double u = (x[i] - mu) * ih, u2 = u * u, u3 = u2 * u;
+        sc[0] = fma(u3, u3, sc[0]); sc[1] = fma(u2, u2, sc[1]); sc[2] = fma(u, u, sc[2]); sc[3] += 1.0;
     }
 #pragma unroll
     for (int a = 0; a < 4; ++a) sc[a] = sqrt(wsum(sc[a]));
@@ -118,8 +123,8 @@ __device__ __forceinline__ bool warp_polyfit3(const double* x, const double* y, 
 #pragma unroll
     for (int a = 0; a < 4; ++a) rhs[a] = 0.0;
     for (int i = lane; i < k; i += 32) {
-        const double v = x[i];
-        const double col[4] = {v * v * v / sc[0], v * v / sc[1], v / sc[2], 1.0 / sc[3]};
+        double col[4];
+        m_cubic_cols((x[i] - mu) * ih, sc, col);
 #pragma unroll
         for (int a = 0; a < 4; ++a) {
             rhs[a] = fma(col[a], y[i], rhs[a]);
@@ -140,8 +145,8 @@ __device__ __forceinline__ bool warp_polyfit3(const double* x, const double* y, 
     for (int it = 0; it < 2; ++it) {
         double r4[4] = {0, 0, 0, 0};
         for (int i = lane; i < k; i += 32) {
-            const double v = x[i];
-            const double col[4] = {v * v * v / sc[0], v * v / sc[1], v / sc[2], 1.0 / sc[3]};
+            double col[4];
+            m_cubic_cols((x[i] - mu) * ih, sc, col);
             const double e = y[i] - (col[0] * sol[0] + col[1] * sol[1] + col[2] * sol[2] + col[3] * sol[3]);
 #pragma unroll
             for (int a = 0; a < 4; ++a) r4[a] = fma(col[a], e, r4[a]);
@@ -153,13 +158,20 @@ __device__ __forceinline__ bool warp_polyfit3(const double* x, const double* y, 
 #pragma unroll
         for (int a = 0; a < 4; ++a) sol[a] += r4[a];
     }
-    if (lane == 0) { coef[0] = sol[0] / sc[0]; coef[1] = sol[1] / sc[1]; coef[2] = sol[2] / sc[2]; coef[3] = sol[3] / sc[3]; }
+#pragma unroll
+    for (int a = 0; a < 4; ++a) sol[a] /= sc[a];
+    double c5[5];
+    m_cubic_from_centred(sol, mu, h, c5);
+    const bool ok = m_coef_finite(c5);
+    if (lane == 0 && ok)
+        for (int a = 0; a < 5; ++a) coef[a] = c5[a];
     __syncwarp();
-    return true;
+    return ok;
 }
 
 // Estimates the Friedrich cubic (feature_calculators.py:131-173 with m = 3): returns in all lanes
-// whether a coefficient vector exists; coefficients land in coef[0..3] (shared memory).
+// whether a coefficient vector exists; coefficients land in coef[0..3], max_langevin_fixed_point in coef[4]
+// (shared memory).
 __device__ __forceinline__ bool friedrich_fit(const float* xs, const float* srt, int n, int r, double* scr, double* coef,
                                               int lane) {
     const int n1 = n - 1;                        // length of signal = x[:-1]
@@ -225,9 +237,10 @@ __device__ __forceinline__ bool friedrich_fit(const float* xs, const float* srt,
     if (k >= 4) ok = warp_polyfit3(sx, sy, k, coef, lane) ? 1 : 0;
     else {
         if (lane == 0) {
-            double c4[4];
-            ok = (k > 0 && m_polyfit3(sx, sy, k, c4)) ? 1 : 0;
-            if (ok) { coef[0] = c4[0]; coef[1] = c4[1]; coef[2] = c4[2]; coef[3] = c4[3]; }
+            double c5[5];
+            ok = m_polyfit3_minnorm(sx, sy, k, c5) ? 1 : 0;
+            if (ok)
+                for (int a = 0; a < 5; ++a) coef[a] = c5[a];
         }
         ok = __shfl_sync(FULL, ok, 0);
     }
@@ -450,7 +463,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                     }
                     if (!fr_ok) { r = dnan(); break; }
                     if (d.calc == TSFX_FRIEDRICH_COEFFICIENTS) r = (d.i0 >= 0 && d.i0 <= 3) ? coef[d.i0] : dnan();
-                    else r = m_poly3_max_real_root(coef[0], coef[1], coef[2], coef[3]);
+                    else r = coef[4];
                     break;
                 }
                 default: break;

@@ -245,76 +245,141 @@ TSFX_HD double m_poly3_max_real_root(double c0, double c1, double c2, double c3)
 }
 
 // ------------------------------------------------------------------ cubic least squares (np.polyfit deg 3)
-// Fits y ~ c0 x^3 + c1 x^2 + c2 x + c3 to k points the way np.polyfit does: Vandermonde columns scaled
-// to unit 2-norm, least squares, minimum-norm solution when k < 4.  Householder-free: modified
-// Gram-Schmidt on the scaled columns (k >= 4) or on the rows (k < 4).  x,y are not modified.
-// Returns false when the problem is numerically rank deficient beyond what polyfit would also flag.
-TSFX_HD bool m_polyfit3(const double* x, const double* y, int k, double* coef /*4*/) {
-    if (k <= 0) return false;
-    double scale[4] = {0, 0, 0, 0};
+// np.polyfit(x, y, 3) scales the Vandermonde columns [x^3, x^2, x, 1] to unit 2-norm and solves by least squares,
+// minimum-norm when k < 4.  For k >= 4 the answer is unique, so it is computed in the centred variable
+// u = (x - mu) / h, mu and h the midpoint and half-width of the points' range: the scaled Vandermonde of u in [-1, 1] is
+// well conditioned whatever the level of x, while that of raw x has a condition number growing like (level/spread)^3,
+// which normal equations would square (NaN or wrong coefficients for series hovering around 300).  The fit in u is then
+// expanded to monomial coefficients of x.  For k < 4 the minimum-norm solution depends on the basis, so it stays in
+// numpy's column-scaled monomial basis, solved by a Householder LQ of the k x 4 matrix.
+
+// mu, h of the centred variable for points in [lo, hi]; false when they do not span a positive, finite range
+TSFX_HD bool m_cubic_centre(double lo, double hi, double* mu, double* h) {
+    *mu = 0.5 * lo + 0.5 * hi;
+    *h = 0.5 * hi - 0.5 * lo;
+    return *h > 0.0 && *h < INFINITY && *mu == *mu;
+}
+
+// column-scaled centred basis [u^3, u^2, u, 1] / sc
+TSFX_HD void m_cubic_cols(double u, const double* sc, double* col) {
+    const double u2 = u * u;
+    col[0] = u2 * u / sc[0]; col[1] = u2 / sc[1]; col[2] = u / sc[2]; col[3] = 1.0 / sc[3];
+}
+
+// a[0..3]: coefficients of u^3 .. u^0.  coef[0..3] = monomial coefficients of x (np.polyfit order), coef[4] =
+// np.max(np.real(np.roots(coef[0..3]))) taken as mu + h * (largest real part of the u-cubic's roots): x -> u is
+// increasing and affine, and leading zeros of the two coefficient vectors coincide.
+TSFX_HD void m_cubic_from_centred(const double* a, double mu, double h, double* coef /*5*/) {
+    double b[4];
+    double hp = 1.0;
+    for (int j = 3; j >= 0; --j) { b[j] = a[j] / hp; hp *= h; }   // polynomial in d = x - mu
+    for (int i = 0; i < 3; ++i)                                    // Taylor shift: q(x - mu) by synthetic division
+        for (int j = 1; j < 4 - i; ++j) b[j] -= mu * b[j - 1];
+    for (int j = 0; j < 4; ++j) coef[j] = b[j];
+    coef[4] = mu + h * m_poly3_max_real_root(a[0], a[1], a[2], a[3]);
+}
+
+TSFX_HD bool m_coef_finite(const double* coef) {
+    for (int c = 0; c < 4; ++c)
+        if (!(fabs(coef[c]) < INFINITY)) return false;
+    return true;
+}
+
+// k < 4 points: A = [L 0] H_{k-1} .. H_0 with Householder reflections H_i acting on columns i..3 from the right; the
+// minimum-norm solution of A w = y is w = H_0 .. H_{k-1} [L^-1 y; 0].  Outputs as m_polyfit3.
+TSFX_HD_NOINLINE bool m_polyfit3_minnorm(const double* x, const double* y, int k, double* coef /*5*/) {
+    if (k <= 0 || k >= 4) return false;
+    double S[4] = {0, 0, 0, 0};
     for (int i = 0; i < k; ++i) {
-        double v = x[i], v2 = v * v, v3 = v2 * v;
-        scale[0] += v3 * v3; scale[1] += v2 * v2; scale[2] += v * v; scale[3] += 1.0;
+        const double v = x[i], v2 = v * v, v3 = v2 * v;
+        S[0] += v3 * v3; S[1] += v2 * v2; S[2] += v * v; S[3] += 1.0;
     }
-    for (int j = 0; j < 4; ++j) scale[j] = sqrt(scale[j]);
-    if (k >= 4) {
-        // normal equations on the scaled columns solved by Cholesky; G is 4x4, well conditioned after
-        // scaling for the binned-mean abscissae this is used on.  One step of iterative refinement.
-        double G[16], rhs[4];
-        for (int a = 0; a < 16; ++a) G[a] = 0.0;
-        for (int a = 0; a < 4; ++a) rhs[a] = 0.0;
+    for (int j = 0; j < 4; ++j) S[j] = sqrt(S[j]);
+    double A[12], V[12], tau[3], w[4] = {0, 0, 0, 0};
+    for (int i = 0; i < k; ++i) {
+        const double v = x[i];
+        A[i * 4 + 0] = v * v * v / S[0]; A[i * 4 + 1] = v * v / S[1];
+        A[i * 4 + 2] = v / S[2];         A[i * 4 + 3] = 1.0 / S[3];
+    }
+    for (int i = 0; i < k; ++i) {
+        double nrm = 0.0;
+        for (int c = i; c < 4; ++c) nrm += A[i * 4 + c] * A[i * 4 + c];
+        nrm = sqrt(nrm);
+        const double alpha = A[i * 4 + i] >= 0.0 ? -nrm : nrm;
+        double vv = 0.0;
+        for (int c = i; c < 4; ++c) { V[i * 4 + c] = A[i * 4 + c] - (c == i ? alpha : 0.0); vv += V[i * 4 + c] * V[i * 4 + c]; }
+        tau[i] = vv > 0.0 ? 2.0 / vv : 0.0;
+        for (int r = i; r < k; ++r) {
+            double s = 0.0;
+            for (int c = i; c < 4; ++c) s += A[r * 4 + c] * V[i * 4 + c];
+            s *= tau[i];
+            for (int c = i; c < 4; ++c) A[r * 4 + c] -= s * V[i * 4 + c];
+        }
+    }
+    for (int i = 0; i < k; ++i) {                 // L z = y; L[i][i] = alpha_i
+        double s = y[i];
+        for (int m = 0; m < i; ++m) s -= A[i * 4 + m] * w[m];
+        w[i] = s / A[i * 4 + i];
+    }
+    for (int i = k - 1; i >= 0; --i) {
+        double s = 0.0;
+        for (int c = i; c < 4; ++c) s += V[i * 4 + c] * w[c];
+        s *= tau[i];
+        for (int c = i; c < 4; ++c) w[c] -= s * V[i * 4 + c];
+    }
+    for (int c = 0; c < 4; ++c) coef[c] = w[c] / S[c];
+    coef[4] = m_poly3_max_real_root(coef[0], coef[1], coef[2], coef[3]);
+    return m_coef_finite(coef);
+}
+
+// Fits the cubic to k points (any order, x, y not modified).  coef[0..3] as np.polyfit(x, y, 3), coef[4] the largest
+// real part of its roots (max_langevin_fixed_point).  Returns false when the data are not finite or the fit is singular.
+TSFX_HD bool m_polyfit3(const double* x, const double* y, int k, double* coef /*5*/) {
+    if (k < 4) return m_polyfit3_minnorm(x, y, k, coef);
+    {
+        double lo = x[0], hi = x[0];
+        for (int i = 1; i < k; ++i) { lo = fmin(lo, x[i]); hi = fmax(hi, x[i]); }
+        double mu, h;
+        if (!m_cubic_centre(lo, hi, &mu, &h)) return false;
+        const double ih = 1.0 / h;
+        double sc[4] = {0, 0, 0, 0};
         for (int i = 0; i < k; ++i) {
-            double v = x[i];
-            double col[4] = {v * v * v / scale[0], v * v / scale[1], v / scale[2], 1.0 / scale[3]};
+            const double u = (x[i] - mu) * ih, u2 = u * u, u3 = u2 * u;
+            sc[0] += u3 * u3; sc[1] += u2 * u2; sc[2] += u * u; sc[3] += 1.0;
+        }
+        for (int j = 0; j < 4; ++j) sc[j] = sqrt(sc[j]);
+        // normal equations of the scaled centred columns (condition number of G below ~1e4 for k >= 4 distinct points
+        // spread over [-1, 1]), Cholesky, two refinement steps with residuals formed from the data
+        double L[16], sol[4];
+        for (int a = 0; a < 16; ++a) L[a] = 0.0;
+        for (int a = 0; a < 4; ++a) sol[a] = 0.0;
+        for (int i = 0; i < k; ++i) {
+            double col[4];
+            m_cubic_cols((x[i] - mu) * ih, sc, col);
             for (int a = 0; a < 4; ++a) {
-                rhs[a] += col[a] * y[i];
-                for (int b = 0; b <= a; ++b) G[a * 4 + b] += col[a] * col[b];
+                sol[a] += col[a] * y[i];
+                for (int b = 0; b <= a; ++b) L[a * 4 + b] += col[a] * col[b];
             }
         }
-        double L[16];
-        for (int a = 0; a < 16; ++a) L[a] = G[a];
         if (!m_cholesky(L, 4, 4)) return false;
-        double sol[4] = {rhs[0], rhs[1], rhs[2], rhs[3]};
         m_forward(L, 4, 4, sol);
         m_backward(L, 4, 4, sol);
-        for (int it = 0; it < 2; ++it) {            // refinement with residual formed from the data
+        for (int it = 0; it < 2; ++it) {
             double r[4] = {0, 0, 0, 0};
             for (int i = 0; i < k; ++i) {
-                double v = x[i];
-                double col[4] = {v * v * v / scale[0], v * v / scale[1], v / scale[2], 1.0 / scale[3]};
-                double e = y[i] - (col[0] * sol[0] + col[1] * sol[1] + col[2] * sol[2] + col[3] * sol[3]);
+                double col[4];
+                m_cubic_cols((x[i] - mu) * ih, sc, col);
+                const double e = y[i] - (col[0] * sol[0] + col[1] * sol[1] + col[2] * sol[2] + col[3] * sol[3]);
                 for (int a = 0; a < 4; ++a) r[a] += col[a] * e;
             }
             m_forward(L, 4, 4, r);
             m_backward(L, 4, 4, r);
             for (int a = 0; a < 4; ++a) sol[a] += r[a];
         }
-        for (int a = 0; a < 4; ++a) coef[a] = sol[a] / scale[a];
-        return true;
+        for (int a = 0; a < 4; ++a) sol[a] /= sc[a];
+        m_cubic_from_centred(sol, mu, h, coef);
     }
-    // k < 4: minimum-norm solution c = A^T (A A^T)^-1 y on the scaled k x 4 matrix
-    double A[12], H[9], z[3];
-    for (int i = 0; i < k; ++i) {
-        double v = x[i];
-        A[i * 4 + 0] = v * v * v / scale[0]; A[i * 4 + 1] = v * v / scale[1];
-        A[i * 4 + 2] = v / scale[2];         A[i * 4 + 3] = 1.0 / scale[3];
-        z[i] = y[i];
-    }
-    for (int i = 0; i < k; ++i)
-        for (int j = 0; j <= i; ++j) {
-            double s = 0.0;
-            for (int c = 0; c < 4; ++c) s += A[i * 4 + c] * A[j * 4 + c];
-            H[i * 3 + j] = s;
-        }
-    if (!m_cholesky(H, k, 3)) return false;
-    m_forward(H, k, 3, z);
-    m_backward(H, k, 3, z);
-    for (int c = 0; c < 4; ++c) {
-        double s = 0.0;
-        for (int i = 0; i < k; ++i) s += A[i * 4 + c] * z[i];
-        coef[c] = s / scale[c];
-    }
-    return true;
+    return m_coef_finite(coef);
 }
 
 // ------------------------------------------------------------------ numpy linear quantile on a sorted array
