@@ -57,6 +57,36 @@ def test_plan_rejects_what_has_no_gpu_path():
     assert p.suffixes == ["ar_coefficient__coeff_1__k_3", "maximum"]
 
 
+def test_plan_parameter_limits():
+    """the largest value the kernels' layouts hold is accepted, the next one refused (DESIGN.md section 1)"""
+    from tsfresh_b200 import plan as P
+    limited = [
+        (lambda v: {"autocorrelation": [{"lag": v}]}, P.MAX_LAG),
+        (lambda v: {"agg_autocorrelation": [{"f_agg": "mean", "maxlag": v}]}, P.MAX_LAG),
+        (lambda v: {"partial_autocorrelation": [{"lag": 3}, {"lag": v}]}, P.MAX_LAG),
+        (lambda v: {"ar_coefficient": [{"coeff": 0, "k": v}]}, P.MAX_AR_K),
+        (lambda v: {"number_cwt_peaks": [{"n": v}]}, P.MAX_CWT_PEAKS_N),
+        (lambda v: {"friedrich_coefficients": [{"coeff": 0, "m": 3, "r": v}]}, P.MAX_FRIEDRICH_R),
+        (lambda v: {"max_langevin_fixed_point": [{"m": 3, "r": v}]}, P.MAX_FRIEDRICH_R),
+        (lambda v: {"permutation_entropy": [{"tau": 1, "dimension": v}]}, P.MAX_PERM_DIMENSION),
+        (lambda v: {"lempel_ziv_complexity": [{"bins": v}]}, P.MAX_LZ_BINS),
+    ]
+    assert (P.MAX_LAG, P.MAX_AR_K, P.MAX_CWT_PEAKS_N, P.MAX_FRIEDRICH_R, P.MAX_PERM_DIMENSION, P.MAX_LZ_BINS) == \
+        (4096, 32, 16, 256, 8, 65535)
+    for make, top in limited:
+        assert Plan(make(top)).n_cols >= 1
+        for over in (top + 1, 100000):
+            with pytest.raises(NotImplementedError, match=r"\(> %d\)" % top):
+                Plan(make(over))
+    # calculators whose lag, n or bins the kernels do not bound
+    p = Plan({"c3": [{"lag": 50000}], "time_reversal_asymmetry_statistic": [{"lag": 50000}], "number_peaks": [{"n": 50000}],
+              "fourier_entropy": [{"bins": 100000}], "binned_entropy": [{"max_bins": 100000}]})
+    assert p.n_cols == 5
+    # the library states the same Lempel-Ziv limit
+    header = open(os.path.join(ROOT, "tsfresh_b200", "csrc", "tsfx_kernels.h")).read()
+    assert re.search(r"#define TSFX_LZ_MAX_BINS (\d+)", header).group(1) == str(P.MAX_LZ_BINS)
+
+
 def test_from_columns_round_trip():
     """from_columns(column names) -> settings whose plan produces exactly those columns (settings.py:23-83; the
     reference pins the same round trip in tests/units/feature_extraction/test_settings.py:100-117)."""

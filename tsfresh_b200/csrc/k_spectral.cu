@@ -256,6 +256,10 @@ __global__ void __launch_bounds__(WPC * 32) k_spectral(SpectralArgs A, int nwtab
             double lmax = -dinf(), lmin = dinf();
             for (int k = lane; k < wnb; k += 32) {
                 double p = pxx[k] / (double)nseg;
+                if (wm == 1) {      // scipy's one-sample window is 1 where the Hann formula gives 0: the detrended sample, squared
+                    const double d0 = (double)xs[0] - (double)xs[0];
+                    p = d0 * d0;
+                }
                 pxx[k] = p;
                 lmax = fmax(lmax, p);
                 lmin = fmin(lmin, p);

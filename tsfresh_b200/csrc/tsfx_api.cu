@@ -481,7 +481,11 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
             case TSFX_APPROXIMATE_ENTROPY:
                 if (d.i0 != 2) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "approximate_entropy: only m=2"); }
                 break;
-            case TSFX_LEMPEL_ZIV_COMPLEXITY: max_lz_bins = std::max(max_lz_bins, d.i0); n_lz += 1; break;
+            case TSFX_LEMPEL_ZIV_COMPLEXITY:
+                // symbols 0 .. bins - 1 are stored in 16 bits, and key (root 0xffff << 16 | symbol 0xffff) is the empty slot
+                if (d.i0 < 1 || d.i0 > TSFX_LZ_MAX_BINS) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "lempel_ziv_complexity: bins must be in 1..65535"); }
+                max_lz_bins = std::max(max_lz_bins, d.i0); n_lz += 1;
+                break;
             case TSFX_PERMUTATION_ENTROPY:
                 if (d.i1 < 2 || d.i1 > 8 || d.i0 < 1) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "permutation_entropy: dimension 2..8, tau >= 1"); }
                 max_perm_dim = std::max(max_perm_dim, d.i1);
@@ -498,6 +502,12 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         }
     }
     if (lag_needed > 4096) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "lag > 4096"); }
+    // k_basic keeps the whole descriptor table in shared memory, wherever the per-warp working sets live
+    if (P->host[G_BASIC].size() > TSFX_BASIC_MAX_COLS &&
+        !std::all_of(P->host[G_BASIC].begin(), P->host[G_BASIC].end(), [](const Desc& d) { return moments_only_calc(d.calc); })) {
+        delete P;
+        return fail(ctx, TSFX_E_UNSUPPORTED, "more than " + std::to_string(TSFX_BASIC_MAX_COLS) + " columns of the BASIC kernel group in one plan");
+    }
     std::vector<int32_t> final_col;
     for (int g = 0; g < G_COUNT; ++g) {
         std::stable_sort(P->host[g].begin(), P->host[g].end(), [g](const Desc& a, const Desc& b) {

@@ -133,6 +133,13 @@ inline int group_max_len(int g) {
 }
 #define G_EVENTS (G_COUNT + 1)      // + the assemble pass
 
+// Plan limits that follow from a layout (tsfx_plan_create refuses larger values with TSFX_E_UNSUPPORTED).
+// lempel_ziv_complexity: symbols are 16-bit and the all-ones key marks an empty slot of the 32-bit key table.
+// BASIC: the CTA-wide descriptor table (40 bytes per column) must fit one CTA's 227 KB next to 1 KB of static shared
+// memory in every placement: 5 632 columns are 220 KB.
+#define TSFX_LZ_MAX_BINS 65535
+#define TSFX_BASIC_MAX_COLS 5632
+
 // Result assembly: every kernel group writes its own dense [n_series x ncols_g] staging matrix (so each
 // 32-byte sector is completed by the warp that owns the row, while it is still in L2); this pass
 // scatters the staging rows into the final row-major [n_series x ncols] matrix in column order.

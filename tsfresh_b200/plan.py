@@ -65,13 +65,24 @@ def _need(name, p, keys):
         raise TypeError("%s() got parameters %s, expected %s" % (name, sorted(p), sorted(keys)))
 
 
-def _int(name, key, v, lo=None):
+def _int(name, key, v, lo=None, hi=None):
     if isinstance(v, (bool, np.bool_)) or int(v) != v:
         _unsupported(name, "%s=%r (integer expected)" % (key, v))
     v = int(v)
     if lo is not None and v < lo:
         raise ValueError("%s: %s=%d must be >= %d" % (name, key, v, lo))
+    if hi is not None and v > hi:
+        _unsupported(name, "%s=%d (> %d)" % (key, v, hi))
     return v
+
+
+# Largest parameter values the kernels' layouts hold (tsfx_plan_create checks the same; DESIGN.md section 1)
+MAX_LAG = 4096              # autocorrelation, agg_autocorrelation maxlag, partial_autocorrelation: lag products per warp
+MAX_AR_K = 32               # ar_coefficient
+MAX_CWT_PEAKS_N = 16        # number_cwt_peaks: rows of the Ricker tap table
+MAX_FRIEDRICH_R = 256       # friedrich_coefficients, max_langevin_fixed_point: quantile bins
+MAX_PERM_DIMENSION = 8      # permutation_entropy: order bits of a window fit 32 bits
+MAX_LZ_BINS = 65535         # lempel_ziv_complexity: 16-bit symbols, and the all-ones key marks an empty slot
 
 
 # ------------------------------------------------------------------------------------------------
@@ -109,9 +120,9 @@ def _simple_with_params(name, p):
         if not (0.0 <= f["p0"] <= 1.0):
             raise ValueError("Quantiles must be in the range [0, 1]")
     elif name in ("autocorrelation", "time_reversal_asymmetry_statistic", "c3"):
-        _need(name, p, ["lag"]); f["i0"] = _int(name, "lag", p["lag"], 0)
+        _need(name, p, ["lag"]); f["i0"] = _int(name, "lag", p["lag"], 0, MAX_LAG if name == "autocorrelation" else None)
     elif name in ("number_cwt_peaks", "number_peaks"):
-        _need(name, p, ["n"]); f["i0"] = _int(name, "n", p["n"], 1)
+        _need(name, p, ["n"]); f["i0"] = _int(name, "n", p["n"], 1, MAX_CWT_PEAKS_N if name == "number_cwt_peaks" else None)
     elif name == "binned_entropy":
         _need(name, p, ["max_bins"]); f["i0"] = _int(name, "max_bins", p["max_bins"], 1)
     elif name == "change_quantiles":
@@ -129,12 +140,10 @@ def _simple_with_params(name, p):
         if f["i0"] != 2:
             _unsupported(name, "m=%d (only m=2)" % f["i0"])
     elif name in ("fourier_entropy", "lempel_ziv_complexity"):
-        _need(name, p, ["bins"]); f["i0"] = _int(name, "bins", p["bins"], 1)
+        _need(name, p, ["bins"]); f["i0"] = _int(name, "bins", p["bins"], 1, MAX_LZ_BINS if name == "lempel_ziv_complexity" else None)
     elif name == "permutation_entropy":
         _need(name, p, ["tau", "dimension"])
-        f["i0"] = _int(name, "tau", p["tau"], 1); f["i1"] = _int(name, "dimension", p["dimension"], 2)
-        if f["i1"] > 8:
-            _unsupported(name, "dimension=%d (> 8)" % f["i1"])
+        f["i0"] = _int(name, "tau", p["tau"], 1); f["i1"] = _int(name, "dimension", p["dimension"], 2, MAX_PERM_DIMENSION)
     elif name == "number_crossing_m":
         _need(name, p, ["m"]); f["p0"] = float(p["m"])
     elif name == "value_count":
@@ -145,7 +154,7 @@ def _simple_with_params(name, p):
         _need(name, p, ["t"]); f["p0"] = float(p["t"])
     elif name == "max_langevin_fixed_point":
         _need(name, p, ["m", "r"])
-        f["i1"] = _int(name, "m", p["m"], 1); f["i2"] = _int(name, "r", p["r"], 1)
+        f["i1"] = _int(name, "m", p["m"], 1); f["i2"] = _int(name, "r", p["r"], 1, MAX_FRIEDRICH_R)
         if f["i1"] != 3:
             _unsupported(name, "m=%d (only the cubic m=3)" % f["i1"])
     else:
@@ -228,10 +237,10 @@ class Plan:
             a = _s_agg("agg_autocorrelation", p["f_agg"], ("mean", "median", "var", "std"))
             yield ('f_agg_"%s"__maxlag_%s' % (p["f_agg"], p["maxlag"]),
                    dict(b, calc=CALC["TSFX_AGG_AUTOCORRELATION"], attr=a,
-                        i0=_int("agg_autocorrelation", "maxlag", p["maxlag"], 0)))
+                        i0=_int("agg_autocorrelation", "maxlag", p["maxlag"], 0, MAX_LAG)))
 
     def _c_partial_autocorrelation(self, plist, b):  # :495
-        top = max(_int("partial_autocorrelation", "lag", p["lag"], 0) for p in plist)
+        top = max(_int("partial_autocorrelation", "lag", p["lag"], 0, MAX_LAG) for p in plist)
         for p in plist:
             yield "lag_%s" % (p["lag"],), dict(b, calc=CALC["TSFX_PARTIAL_AUTOCORRELATION"], i0=int(p["lag"]), i1=top)
 
@@ -283,9 +292,7 @@ class Plan:
 
     def _c_ar_coefficient(self, plist, b):  # :1485-1505
         for p in plist:
-            k = _int("ar_coefficient", "k", p["k"], 1)
-            if k > 32:
-                _unsupported("ar_coefficient", "k=%d (> 32)" % k)
+            k = _int("ar_coefficient", "k", p["k"], 1, MAX_AR_K)
             yield "coeff_%s__k_%s" % (p["coeff"], p["k"]), dict(
                 b, calc=CALC["TSFX_AR_COEFFICIENT"], i0=_int("ar_coefficient", "coeff", p["coeff"], 0), i1=k)
 
@@ -297,7 +304,7 @@ class Plan:
                 _unsupported("friedrich_coefficients", "m=%d (only the cubic m=3)" % m)
             yield "coeff_%s__m_%s__r_%s" % (p["coeff"], p["m"], p["r"]), dict(
                 b, calc=CALC["TSFX_FRIEDRICH_COEFFICIENTS"], i0=int(p["coeff"]), i1=m,
-                i2=_int("friedrich_coefficients", "r", p["r"], 1))
+                i2=_int("friedrich_coefficients", "r", p["r"], 1, MAX_FRIEDRICH_R))
 
     def _c_agg_linear_trend(self, plist, b):  # :2198-2220
         for p in plist:
