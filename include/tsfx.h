@@ -75,7 +75,7 @@ enum tsfx_calc {
     TSFX_SUM_VALUES,                                   /* :371 */
     TSFX_AGG_AUTOCORRELATION,                          /* :387  attr=f_agg i0=maxlag */
     TSFX_PARTIAL_AUTOCORRELATION,                      /* :440  i0=lag i1=max lag over the param list */
-    TSFX_AUGMENTED_DICKEY_FULLER,                      /* :499  attr=teststat|pvalue|usedlag i0=autolag */
+    TSFX_AUGMENTED_DICKEY_FULLER,                      /* :499  attr=teststat|pvalue|usedlag i0=autolag (TSFX_AUTOLAG_*) */
     TSFX_ABS_ENERGY,                                   /* :548 */
     TSFX_CID_CE,                                       /* :567  i0=normalize */
     TSFX_MEAN_ABS_CHANGE,                              /* :604 */
@@ -109,7 +109,7 @@ enum tsfx_calc {
     TSFX_NUMBER_PEAKS,                                 /* :1235 i0=n */
     TSFX_INDEX_MASS_QUANTILE,                          /* :1275 p0=q */
     TSFX_NUMBER_CWT_PEAKS,                             /* :1320 i0=n */
-    TSFX_LINEAR_TREND,                                 /* :1343 attr=pvalue|rvalue|intercept|slope|stderr */
+    TSFX_LINEAR_TREND,                                 /* :1343 attr=pvalue|rvalue|intercept|slope|stderr|intercept_stderr */
     TSFX_CWT_COEFFICIENTS,                             /* :1370 i0=coeff i1=table index of scale w */
     TSFX_SPKT_WELCH_DENSITY,                           /* :1418 i0=coeff */
     TSFX_AR_COEFFICIENT,                               /* :1459 i0=coeff i1=k */
@@ -146,12 +146,20 @@ enum tsfx_calc {
 };
 
 /* attr codes */
-enum { TSFX_AGG_MEAN = 0, TSFX_AGG_MEDIAN, TSFX_AGG_VAR, TSFX_AGG_STD, TSFX_AGG_MAX, TSFX_AGG_MIN };
+/* f_agg: numpy reducers (var and std with ddof 0; ptp = max - min).  agg_linear_trend takes mean, median, var, std, max
+ * and min.  agg_autocorrelation and change_quantiles take every code, and OR'ed with TSFX_AGG_NANSKIP the np.nan*
+ * variant, which skips NaN: on no value left nansum gives 0, nanprod 1 and the others NaN. */
+enum { TSFX_AGG_MEAN = 0, TSFX_AGG_MEDIAN, TSFX_AGG_VAR, TSFX_AGG_STD, TSFX_AGG_MAX, TSFX_AGG_MIN, TSFX_AGG_PTP,
+       TSFX_AGG_SUM, TSFX_AGG_PROD };
+#define TSFX_AGG_NANSKIP 16
 enum { TSFX_FFT_REAL = 0, TSFX_FFT_IMAG, TSFX_FFT_ABS, TSFX_FFT_ANGLE };
 enum { TSFX_SPEC_CENTROID = 0, TSFX_SPEC_VARIANCE, TSFX_SPEC_SKEW, TSFX_SPEC_KURTOSIS };
-enum { TSFX_LR_PVALUE = 0, TSFX_LR_RVALUE, TSFX_LR_INTERCEPT, TSFX_LR_SLOPE, TSFX_LR_STDERR };
+/* linregress attributes; intercept_stderr = stderr * sqrt(ssxm + xmean^2) (scipy.stats.linregress) */
+enum { TSFX_LR_PVALUE = 0, TSFX_LR_RVALUE, TSFX_LR_INTERCEPT, TSFX_LR_SLOPE, TSFX_LR_STDERR, TSFX_LR_INTERCEPT_STDERR };
 enum { TSFX_ADF_TESTSTAT = 0, TSFX_ADF_PVALUE, TSFX_ADF_USEDLAG, TSFX_ADF_BADATTR };
-enum { TSFX_AUTOLAG_AIC = 0, TSFX_AUTOLAG_BIC, TSFX_AUTOLAG_NONE };
+/* adfuller autolag: AIC / BIC (smallest criterion), TSTAT ("t-stat": from the longest model down, the first whose last
+ * lag has |t| >= 1.6448536269514722, else no lag), NONE (maxlag) */
+enum { TSFX_AUTOLAG_AIC = 0, TSFX_AUTOLAG_BIC, TSFX_AUTOLAG_NONE, TSFX_AUTOLAG_TSTAT };
 
 /* One output column. `col` is its index in the row-major [n_series x n_cols] result. */
 typedef struct tsfx_feature_desc {

@@ -266,6 +266,75 @@ __device__ __forceinline__ double agg_chunk(const float* xs, int lo, int hi, int
     return f_agg == TSFX_AGG_STD ? sqrt(v) : v;
 }
 
+// The parameter values beyond the Comprehensive grid, in a call of its own after the descriptor trip that wrote the run's
+// columns (k_basic<..., VOCAB = true>, which the launcher runs only for plans that have one).  It overwrites what the trip wrote for
+//   agg_autocorrelation with a reducer other than mean / median / var / std (np_stats / np_finish over the lag vector),
+//   attr intercept_stderr of linear_trend, linear_trend_timewise and agg_linear_trend (the fit again, from the same sums).
+// out: the run's columns, or nullptr for a duplicate row that only keeps the CTA's warps in step.
+__device__ __noinline__ void basic_vocabulary(const Desc* d, int run, const double* xc, double* scr, const double* lagS,
+                                              const double* altS, int n, double mean, double var, bool have_times,
+                                              double* out, int lane) {
+    const double dn = (double)n;
+    switch (d[0].calc) {
+        case TSFX_AGG_AUTOCORRELATION: {
+            if (d[0].attr <= TSFX_AGG_STD) return;
+            const bool zero = (fabs(var) < 1e-10) || n == 1;
+            const int cnt = max(zero ? min(d[0].i0, n) : min(d[0].i0, n - 1), 0);
+            double r = 0.0;                                     // a = [0] * n
+            if (!zero || cnt == 0) {                            // cnt == 0 (maxlag 0): numpy on an empty array
+                if (!zero) {
+                    const double a0 = lagS[0] / dn;
+                    for (int k = 1 + lane; k <= cnt; k += 32) scr[k - 1] = (lagS[k] / (double)(n - k)) / a0;
+                    __syncwarp();
+                }
+                const auto get = [&](int i, double& x) { x = scr[i]; return true; };
+                r = np_finish(np_stats(get, cnt, lane), get, cnt, d[0].attr, lane);
+            }
+            if (lane == 0 && out) out[0] = r;
+            return;
+        }
+        case TSFX_LINEAR_TREND:
+        case TSFX_LINEAR_TREND_TIMEWISE: {
+            // the regressor: 0 .. n-1, or the hours since the first row that the trip staged in scr
+            const bool tw = d[0].calc == TSFX_LINEAR_TREND_TIMEWISE;
+            if (tw && !have_times) return;
+            double tm = 0.5 * (double)(n - 1);
+            if (tw) {
+                double st = 0.0;
+                for (int i = lane; i < n; i += 32) st += scr[i];
+                tm = wsum(st) / dn;
+            }
+            double sxx = 0.0, sxy = 0.0;
+            for (int i = lane; i < n; i += 32) {
+                const double dt = (tw ? scr[i] : (double)i) - tm;
+                sxx = fma(dt, dt, sxx);
+                sxy = fma(dt, xc[i], sxy);
+            }
+            sxx = wsum(sxx) / dn;
+            sxy = wsum(sxy) / dn;
+            const double se = m_intercept_stderr(m_linregress(dn, tm, mean, sxx, var, sxy).stderr_, tm, sxx);
+            if (out)
+                for (int t = lane; t < run; t += 32)
+                    if (d[t].attr == TSFX_LR_INTERCEPT_STDERR) out[t] = se;
+            return;
+        }
+        case TSFX_AGG_LINEAR_TREND: {
+            // stage A's slot of every (chunk_len, f_agg) key, in the same order
+            int slot = -1, prev = -1;
+            for (int t = 0; t < run; ++t) {
+                const int key = (d[t].i0 << 4) | d[t].i1;
+                if (key != prev) { ++slot; prev = key; }
+                if (lane != 0 || !out || d[t].attr != TSFX_LR_INTERCEPT_STDERR) continue;
+                const double* S = altS + 6 * slot;
+                out[t] = S[0] >= 0.0 ? m_intercept_stderr(m_linregress(S[0], S[1], S[2], S[3], S[4], S[5]).stderr_, S[1], S[3])
+                                     : dnan();
+            }
+            return;
+        }
+        default: return;
+    }
+}
+
 // the inputs of linregress(range(k), y[0..k)) with y in shared memory: k, mean(t), mean(y), ssxm, ssym, ssxym
 struct LinSums { double k, tm, ym, sxx, syy, sxy; };
 __device__ __forceinline__ LinSums linreg_sums(const double* y, int k, int lane) {
@@ -399,7 +468,9 @@ __device__ __noinline__ double basic_finisher(const Desc& d, const double* ST, c
     }
 }
 
-template <int WPC, bool GS>
+// VOCAB: the instantiation for plans with a column basic_vocabulary finishes (launch_basic's vocab); without it the kernel
+// is as it was before those columns existed, so the plans that do not ask for them keep its register allocation
+template <int WPC, bool GS, bool VOCAB>
 __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))) k_basic(BasicArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -884,6 +955,11 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                 default: r = dnan(); break;
             }
             if (!stored && lane == 0 && live) orow[j] = r;
+            if (VOCAB) {
+                __syncwarp();
+                basic_vocabulary(sdesc + j, used, xc, scr, lagS, altS, n, M.mean, M.var, A.R.times != nullptr,
+                                 live ? orow + j : nullptr, lane);
+            }
             j += used;
         }
         __syncwarp();
@@ -893,7 +969,7 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
 bool basic_finisher_calc(int calc) { return basic_is_finisher(calc); }
 
 // ------------------------------------------------------------------------------------------ launcher
-cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+cudaError_t launch_basic(const BasicArgs& A0, bool vocab, int max_len, cudaStream_t st, int sm_count, const char** variant) {
     BasicArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     A.nscr = std::max(A.nscr, (max_len + 1) & ~1);      // the plan's scratch need, at least the series
@@ -926,7 +1002,11 @@ cudaError_t launch_basic(const BasicArgs& A0, int max_len, cudaStream_t st, int 
         G.smem = per * 12 + A.desc_bytes;
         G.grid = cta_grid(A.R.n_series, 12, (int64_t)sm_count * grid_waves(4096));
     }
-    auto launch = [&](auto g) { return launch_kernel(k_basic<decltype(g)::wpc, decltype(g)::global>, G, st, A); };
+    auto launch = [&](auto g) {
+        constexpr int W = decltype(g)::wpc;
+        constexpr bool GL = decltype(g)::global;
+        return vocab ? launch_kernel(k_basic<W, GL, true>, G, st, A) : launch_kernel(k_basic<W, GL, false>, G, st, A);
+    };
     TSFX_LAUNCH_DECLARED(TSFX_GEOMS_BASIC, "basic", G, variant, launch);
 }
 

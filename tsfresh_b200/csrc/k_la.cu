@@ -1,7 +1,7 @@
 // k_la.cu -- kernel group LA: small dense least-squares problems per series.
 //   ar_coefficient          (feature_calculators.py:1459-1507; statsmodels AutoReg(lags=k, trend="c") OLS)
 //   augmented_dickey_fuller (feature_calculators.py:499-544; statsmodels adfuller(regression="c"),
-//                            autolag AIC / BIC / None) -- restated in oracle/thirdparty.py
+//                            autolag AIC / BIC / t-stat / None) -- restated in oracle/thirdparty.py
 //
 // One warp per series.  Normal equations are formed cooperatively (one Gram entry per lane, looping over
 // the rows) on mean-centred regressors, then solved by lane 0 with a float64 Cholesky.  The nested ADF
@@ -92,7 +92,51 @@ __device__ __forceinline__ void warp_backward(const double* L, int q, int lda, d
     }
 }
 
-template <int WPC, bool GS>
+// ADF autolag "t-stat" (statsmodels adfuller): from the longest model down, the first whose last regressor has
+// |t| >= 1.6448536269514722 gives usedlag = its lag count; none: 0.  The same autolag Gram and factorisation as the AIC /
+// BIC search, in a call of its own so that the kernel's search compiles as it does without it.  With z = L^-1 X'y the t
+// value of model q's last coefficient is z_{q-1} / sqrt(SSR_q / (nobs - q)); lane 0 keeps it in bvec[q-1].
+__device__ __noinline__ int adf_tstat_lag(const double* dx, const double* xc, int n, int M0, double* Pm, double* Cv,
+                                          double* Lv, double* G, double* bvec, int pmax, int lane) {
+    const int nd_ = n - 1, p = M0 + 2, t0 = M0, nobs = nd_ - M0;
+    lag_gram(dx, xc, t0, nd_, M0, Pm, pmax, Cv, Lv, lane);
+    double l1 = 0.0, l2 = 0.0;
+    for (int t = t0 + lane; t < nd_; t += 32) { double v = xc[t]; l1 += v; l2 = fma(v, v, l2); }
+    l1 = wsum(l1); l2 = wsum(l2);
+    for (int e = lane; e < p * p; e += 32) {
+        const int a = e / p, c = e - a * p;
+        if (c > a) continue;
+        double v;
+        if (a == 0) v = (double)nobs;
+        else if (a == 1) v = (c == 0) ? l1 : l2;
+        else v = (c == 0) ? Cv[a - 1] : (c == 1 ? Lv[a - 1] : Pm[(a - 1) * pmax + (c - 1)]);
+        G[a * p + c] = v;
+    }
+    for (int a = lane; a < p; a += 32) bvec[a] = (a == 0) ? Cv[0] : (a == 1 ? Lv[0] : Pm[(a - 1) * pmax + 0]);
+    const double yy = Pm[0];
+    __syncwarp();
+    const int okq = warp_cholesky(G, p, p, lane);
+    double ssr = yy;
+    const double dnobs = (double)nobs;
+    for (int i = 0; i < okq; ++i) {
+        const double z = bvec[i] / G[i * p + i];
+        __syncwarp();
+        for (int r2 = i + 1 + lane; r2 < okq; r2 += 32) bvec[r2] = fma(-G[r2 * p + i], z, bvec[r2]);
+        __syncwarp();
+        ssr -= z * z;
+        if (lane == 0) bvec[i] = z / sqrt(ssr / (dnobs - (double)(i + 1)));
+    }
+    __syncwarp();
+    int used = 0;
+    for (int q = okq; q > 2; --q)
+        if (fabs(bvec[q - 1]) >= 1.6448536269514722) { used = q - 2; break; }
+    __syncwarp();
+    return used;
+}
+
+// TSTAT: the instantiation for plans with autolag "t-stat" (adf_tstat_lag); without it the kernel is as it was before
+// that mode existed, so the plans that do not ask for it keep its register allocation
+template <int WPC, bool GS, bool TSTAT>
 __global__ void __launch_bounds__(WPC * 32) k_la(LaArgs A, int pmax) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -169,7 +213,9 @@ __global__ void __launch_bounds__(WPC * 32) k_la(LaArgs A, int pmax) {
                     if (M.vmax != M.vmin && M0 >= 0) {
                         const int nd_ = n - 1;
                         int used = M0;
-                        if (adf_mode != TSFX_AUTOLAG_NONE) {
+                        if (TSTAT && adf_mode == TSFX_AUTOLAG_TSTAT) {
+                            used = adf_tstat_lag(dx, xc, n, M0, Pm, Cv, Lv, G, bvec, pmax, lane);
+                        } else if (adf_mode != TSFX_AUTOLAG_NONE) {
                             const int p = M0 + 2, t0 = M0, nobs = nd_ - M0;
                             double* yy = res + 7;
                             // columns [const, level, dlag1..dlagM]; y = dx[t] = "dlag0"
@@ -477,7 +523,7 @@ __device__ __forceinline__ void adf_gram(const double* xs, int n, int M0, double
     __syncwarp();
 }
 
-template <int WPC, int MINB>
+template <int WPC, int MINB, bool TSTAT>     // TSTAT: as for k_la
 __global__ void __launch_bounds__(WPC * 32, MINB) k_la_small(LaArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -573,28 +619,42 @@ __global__ void __launch_bounds__(WPC * 32, MINB) k_la_small(LaArgs A) {
                                 ssr -= z * z;
                                 if (lane == i) ssr_q = ssr;
                             }
-                            // information criterion of every nested model, one model per lane, then the reference's
-                            // first-minimum scan in model order
-                            double ic = 0.0;
-                            const int q = lane + 1;
-                            if (q >= 2 && q <= okq) {
-                                const double llf = -dnobs / 2.0 * log(2.0 * 3.14159265358979323846) -
-                                                   dnobs / 2.0 * log(ssr_q / dnobs) - dnobs / 2.0;
-                                const double pen = (adf_mode == TSFX_AUTOLAG_AIC) ? 2.0 * (double)q : log(dnobs) * (double)q;
-                                ic = -2.0 * llf + pen;
+                            if (TSTAT && adf_mode == TSFX_AUTOLAG_TSTAT) {
+                                // t-stat: the t value of every nested model's last regressor, z_{q-1} / sqrt(SSR_q /
+                                // (nobs - q)), one model per lane, then the scan from the longest model down (as in k_la)
+                                const int q = lane + 1;
+                                const double t = (q >= 2 && q <= okq) ? cb[lane] / sqrt(ssr_q / (dnobs - (double)q)) : 0.0;
+                                __syncwarp();
+                                cb[lane] = t;
+                                __syncwarp();
+                                used = 0;
+                                for (int qq = okq; qq > 2; --qq)
+                                    if (fabs(cb[qq - 1]) >= 1.6448536269514722) { used = qq - 2; break; }
+                                __syncwarp();
+                            } else {
+                                // information criterion of every nested model, one model per lane, then the reference's
+                                // first-minimum scan in model order
+                                double ic = 0.0;
+                                const int q = lane + 1;
+                                if (q >= 2 && q <= okq) {
+                                    const double llf = -dnobs / 2.0 * log(2.0 * 3.14159265358979323846) -
+                                                       dnobs / 2.0 * log(ssr_q / dnobs) - dnobs / 2.0;
+                                    const double pen = (adf_mode == TSFX_AUTOLAG_AIC) ? 2.0 * (double)q : log(dnobs) * (double)q;
+                                    ic = -2.0 * llf + pen;
+                                }
+                                __syncwarp();
+                                cb[lane] = ic;
+                                __syncwarp();
+                                int best_q = 2;
+                                double best_ic = 0.0;
+                                bool have = false;
+                                for (int qq = 2; qq <= okq; ++qq) {
+                                    const double icq = cb[qq - 1];
+                                    if (!have || icq < best_ic) { have = true; best_ic = icq; best_q = qq; }
+                                }
+                                __syncwarp();
+                                used = best_q - 2;
                             }
-                            __syncwarp();
-                            cb[lane] = ic;
-                            __syncwarp();
-                            int best_q = 2;
-                            double best_ic = 0.0;
-                            bool have = false;
-                            for (int qq = 2; qq <= okq; ++qq) {
-                                const double icq = cb[qq - 1];
-                                if (!have || icq < best_ic) { have = true; best_ic = icq; best_q = qq; }
-                            }
-                            __syncwarp();
-                            used = best_q - 2;
                         }
                         // final regression on the longer sample [used, nd_): the autolag Gram's columns
                         // [const, dlag1..dlagU, level, y] plus the rows t = used .. M0-1 as rank-one updates
@@ -637,15 +697,16 @@ __global__ void __launch_bounds__(WPC * 32, MINB) k_la_small(LaArgs A) {
     }
 }
 
-cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+cudaError_t launch_la(const LaArgs& A0, bool tstat, int max_len, cudaStream_t st, int sm_count, const char** variant) {
     LaArgs A = A0;
     if (max_len <= LA_SMALL_LEN && A.max_ar_k <= LA_SMALL_KMAX) {
         A.npad = LA_SMALL_LEN;
         A.bytes_per_warp = (LA_SMALL_LEN + LA_SMALL_P * LA_SMALL_LD + LA_SMALL_CB + 32) * 8;
         A.gscratch = nullptr;
         *variant = "la/small";
-        return launch_fixed(k_la_small<LA_SMALL_WPC, 3>, LA_SMALL_WPC * 32, LA_SMALL_WPC, (size_t)A.bytes_per_warp * LA_SMALL_WPC,
-                            (int64_t)sm_count * grid_waves(4096), A.R.n_series, st, A);
+        return launch_fixed(tstat ? k_la_small<LA_SMALL_WPC, 3, true> : k_la_small<LA_SMALL_WPC, 3, false>, LA_SMALL_WPC * 32,
+                            LA_SMALL_WPC, (size_t)A.bytes_per_warp * LA_SMALL_WPC, (int64_t)sm_count * grid_waves(4096),
+                            A.R.n_series, st, A);
     }
     A.npad = (max_len + 3) & ~3;
     // autolag keeps one model per lane in three rounds: 96 models, maxlag 73 (75 models) at TSFX_L_MAX
@@ -658,7 +719,11 @@ cudaError_t launch_la(const LaArgs& A0, int max_len, cudaStream_t st, int sm_cou
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    auto launch = [&](auto g) { return launch_kernel(k_la<decltype(g)::wpc, decltype(g)::global>, G, st, A, pmax); };
+    auto launch = [&](auto g) {
+        constexpr int W = decltype(g)::wpc;
+        constexpr bool GL = decltype(g)::global;
+        return tstat ? launch_kernel(k_la<W, GL, true>, G, st, A, pmax) : launch_kernel(k_la<W, GL, false>, G, st, A, pmax);
+    };
     TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "la", G, variant, launch);
 }
 

@@ -56,6 +56,42 @@ __device__ __forceinline__ double wsum8_scatter(const double (&v)[8], int lane) 
     return c;
 }
 
+// change_quantiles columns whose reducer is not mean, var or std -- the corridor sweep's statistics -- in a call of its own
+// after the sweep, so that the sweep compiles as it does without them (tsfx_plan_create sets SortedArgs::cq_own only for
+// plans that have one).  Descriptors of one corridor and isabs are adjacent (tsfx_plan_create's order), and they share one
+// np_stats sweep over the changes whose both ends lie in the corridor -- the same float32 bounds as the sweep's; var, std
+// and the median sweep again.  0.0 where the reference returns before aggregating (ql >= qh, no change inside).
+// Differences of two float32 samples are exact in float64 unless their exponents lie more than 29 apart, so max and min
+// are the reference's bits.  out: the run's columns, or nullptr for a duplicate row.
+__device__ __noinline__ void cq_own_passes(const Desc* descs, int run, const float* xs, const float* srt, int n, double* out,
+                                           int lane) {
+    NpStats S = {0, 0, 0.0, 1.0, 0.0, 0.0};
+    float lo = 0.f, hi = 0.f;
+    bool isabs = false, have = false;
+    double pl = 0.0, ph = 0.0;
+    const auto get = [&](int i, double& x) {
+        const float a = xs[i], b = xs[i + 1];
+        x = (double)b - (double)a;
+        if (isabs) x = fabs(x);
+        return a >= lo && a <= hi && b >= lo && b <= hi;
+    };
+    for (int t = 0; t < run; ++t) {
+        const Desc e = descs[t];
+        if (e.attr == TSFX_AGG_MEAN || e.attr == TSFX_AGG_VAR || e.attr == TSFX_AGG_STD) continue;
+        double r = 0.0;
+        if (e.p0 < e.p1) {
+            if (!have || e.p0 != pl || e.p1 != ph || (e.i0 != 0) != isabs) {
+                have = true; pl = e.p0; ph = e.p1; isabs = e.i0 != 0;
+                lo = __double2float_ru(m_quantile_sorted(srt, n, e.p0));
+                hi = __double2float_rd(m_quantile_sorted(srt, n, e.p1));
+                S = np_stats(get, n - 1, lane);
+            }
+            if (S.c + S.nans > 0) r = np_finish(S, get, n - 1, e.attr, lane);
+        }
+        if (lane == 0 && out) out[t] = r;
+    }
+}
+
 struct Uniq { int n_unique, n_reocc_values, n_reocc_points; double sum_reocc_values, sum_reocc_points; bool any_dup; };
 
 __device__ __forceinline__ Uniq unique_pass(const float* s, int n, int lane) {
@@ -248,7 +284,9 @@ __device__ __forceinline__ bool friedrich_fit(const float* xs, const float* srt,
     return ok != 0;
 }
 
-template <int WPC, bool GS>
+// CQ_OWN: the instantiation for plans with a change_quantiles reducer cq_own_passes computes; without it the kernel is as
+// it was before those reducers existed, so the plans that do not ask for them keep its register allocation
+template <int WPC, bool GS, bool CQ_OWN>
 __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))) k_sorted(SortedArgs A) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -469,6 +507,10 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                 default: break;
             }
             if (!stored && lane == 0 && live) orow[j] = r;
+            if (CQ_OWN && d.calc == TSFX_CHANGE_QUANTILES) {
+                __syncwarp();
+                cq_own_passes(A.descs + j, used, xs, srt, n, live ? orow + j : nullptr, lane);
+            }
             j += used;
         }
         __syncwarp();
@@ -486,7 +528,7 @@ bool sorted_finisher_calc(int calc) {
     }
 }
 
-cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, int sm_count, const char** variant) {
+cudaError_t launch_sorted(const SortedArgs& A0, bool cq_own, int max_len, cudaStream_t st, int sm_count, const char** variant) {
     SortedArgs A = A0;
     A.npad = (max_len + 3) & ~3;
     int p2 = 1;
@@ -498,7 +540,11 @@ cudaError_t launch_sorted(const SortedArgs& A0, int max_len, cudaStream_t st, in
     Geometry G;
     if (!plan_geometry(per, 100 * 1024, 8, A.R.n_series, sm_count, A.gscratch, A.gscratch_bytes, &G)) return cudaErrorInvalidConfiguration;
     A.gscratch = G.gscratch;
-    auto launch = [&](auto g) { return launch_kernel(k_sorted<decltype(g)::wpc, decltype(g)::global>, G, st, A); };
+    auto launch = [&](auto g) {
+        constexpr int W = decltype(g)::wpc;
+        constexpr bool GL = decltype(g)::global;
+        return cq_own ? launch_kernel(k_sorted<W, GL, true>, G, st, A) : launch_kernel(k_sorted<W, GL, false>, G, st, A);
+    };
     TSFX_LAUNCH_DECLARED(TSFX_GEOMS_ALL, "sorted", G, variant, launch);
 }
 

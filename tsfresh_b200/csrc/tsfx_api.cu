@@ -278,6 +278,9 @@ struct tsfx_plan {
     Desc* dev[G_COUNT] = {nullptr};
     int32_t* d_final_col = nullptr;   // final column of every staged column, groups concatenated
     double2* d_cq = nullptr;          // (ql, qh) of the distinct change_quantiles corridors (SortedArgs::cq)
+    bool sorted_cq_own = false;       // SORTED runs the instantiation with cq_own_passes (launch_sorted)
+    bool basic_vocab = false;         // BASIC runs the instantiation with basic_vocabulary (launch_basic)
+    bool la_tstat = false;            // LA runs the instantiations with the t-stat lag search (launch_la)
     bool basic_moments_only = false;  // the BASIC group is reductions only: k_moments replaces k_basic
     int moments_need_high = 0;
     int n_groups_used = 0;
@@ -437,6 +440,14 @@ extern "C" int tsfx_sync(tsfx_ctx* ctx) {
 // ------------------------------------------------------------------------------------------ plan
 static int even(int v) { return (v + 1) & ~1; }
 
+// f_agg codes of agg_autocorrelation and change_quantiles: TSFX_AGG_MEAN .. TSFX_AGG_PROD, each also with TSFX_AGG_NANSKIP
+// (np.average is TSFX_AGG_MEAN; there is no nanptp or nanaverage in numpy)
+static bool numpy_agg_code(int a) {
+    const int op = a & ~TSFX_AGG_NANSKIP;
+    if (a < 0 || op > TSFX_AGG_PROD) return false;
+    return !(a & TSFX_AGG_NANSKIP) || op != TSFX_AGG_PTP;
+}
+
 extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, int32_t n_descs, int32_t n_cols,
                                 const double* tables, const int64_t* table_off, const int32_t* table_half,
                                 int32_t n_tables, tsfx_plan** out) {
@@ -461,7 +472,25 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         P->host[group_of(d.calc)].push_back(d);
         switch (d.calc) {
             case TSFX_AUTOCORRELATION: lag_needed = std::max(lag_needed, d.i0); break;
-            case TSFX_AGG_AUTOCORRELATION: lag_needed = std::max(lag_needed, d.i0); break;
+            case TSFX_AGG_AUTOCORRELATION:
+                if (!numpy_agg_code(d.attr)) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "agg_autocorrelation: unknown f_agg code"); }
+                lag_needed = std::max(lag_needed, d.i0);
+                break;
+            case TSFX_CHANGE_QUANTILES:
+                if (!numpy_agg_code(d.attr)) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "change_quantiles: unknown f_agg code"); }
+                break;
+            case TSFX_LINEAR_TREND:
+                if (d.attr < 0 || d.attr > TSFX_LR_INTERCEPT_STDERR) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "linear_trend: unknown attr code"); }
+                break;
+            case TSFX_AGG_LINEAR_TREND:
+                if (d.attr < 0 || d.attr > TSFX_LR_INTERCEPT_STDERR || d.i1 < TSFX_AGG_MEAN || d.i1 > TSFX_AGG_MIN) {
+                    delete P;
+                    return fail(ctx, TSFX_E_UNSUPPORTED, "agg_linear_trend: unknown attr or f_agg code");
+                }
+                break;
+            case TSFX_AUGMENTED_DICKEY_FULLER:
+                if (d.i0 < TSFX_AUTOLAG_AIC || d.i0 > TSFX_AUTOLAG_TSTAT) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "augmented_dickey_fuller: unknown autolag code"); }
+                break;
             case TSFX_PARTIAL_AUTOCORRELATION:
                 lag_needed = std::max(lag_needed, d.i1);
                 pacf_want = std::max(pacf_want, d.i1);
@@ -477,7 +506,10 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
                 if (d.i1 < 1 || d.i1 > 32) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "ar_coefficient: k must be in 1..32"); }
                 max_ar_k = std::max(max_ar_k, d.i1);
                 break;
-            case TSFX_LINEAR_TREND_TIMEWISE: P->need_times = 1; break;
+            case TSFX_LINEAR_TREND_TIMEWISE:
+                if (d.attr < 0 || d.attr > TSFX_LR_INTERCEPT_STDERR) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "linear_trend_timewise: unknown attr code"); }
+                P->need_times = 1;
+                break;
             case TSFX_APPROXIMATE_ENTROPY:
                 if (d.i0 != 2) { delete P; return fail(ctx, TSFX_E_UNSUPPORTED, "approximate_entropy: only m=2"); }
                 break;
@@ -587,6 +619,9 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
         const Desc& d = P->host[G_BASIC][q];
         const int key = (d.i0 << 4) | d.i1;
         if (d.calc == TSFX_AGG_LINEAR_TREND && key != prev) { ++B.nalt; prev = key; }
+        if (((d.calc == TSFX_LINEAR_TREND || d.calc == TSFX_LINEAR_TREND_TIMEWISE || d.calc == TSFX_AGG_LINEAR_TREND) &&
+             d.attr == TSFX_LR_INTERCEPT_STDERR) || (d.calc == TSFX_AGG_AUTOCORRELATION && d.attr > TSFX_AGG_STD))
+            P->basic_vocab = true;
     }
     B.dec = ctx->d_dec;
     SortedArgs& S = P->sorted;
@@ -598,6 +633,9 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
     for (const Desc& d : P->host[G_SORTED])
         if (d.calc == TSFX_CHANGE_QUANTILES && !(d.p0 == pl && d.p1 == ph)) { cq.push_back(make_double2(d.p0, d.p1)); pl = d.p0; ph = d.p1; }
     S.ncq = (int)cq.size();
+    for (const Desc& d : P->host[G_SORTED])
+        if (d.calc == TSFX_CHANGE_QUANTILES && d.attr != TSFX_AGG_MEAN && d.attr != TSFX_AGG_VAR && d.attr != TSFX_AGG_STD)
+            P->sorted_cq_own = true;
     if (!cq.empty()) {
         cudaError_t e = cudaMalloc(&P->d_cq, cq.size() * sizeof(double2));
         if (e == cudaSuccess) e = cudaMemcpy(P->d_cq, cq.data(), cq.size() * sizeof(double2), cudaMemcpyHostToDevice);
@@ -612,6 +650,8 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
     F.nfft = spectral_nfft;
     group(P->la, G_LA);
     P->la.max_ar_k = max_ar_k;
+    for (const Desc& d : P->host[G_LA])
+        if (d.calc == TSFX_AUGMENTED_DICKEY_FULLER && d.i0 == TSFX_AUTOLAG_TSTAT) P->la_tstat = true;
     group(P->entropy, G_ENTROPY);
     SeqArgs& Q = P->seq;
     group(Q, G_SEQ);
@@ -761,17 +801,17 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
                     ctx->used_moments = true;
                     break;
                 }
-                e = launch_basic(call(P->basic), max_len, gs, ctx->sm_count, &variant);
+                e = launch_basic(call(P->basic), P->basic_vocab, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
-            case G_SORTED: e = launch_sorted(call(P->sorted), max_len, gs, ctx->sm_count, &variant); break;
+            case G_SORTED: e = launch_sorted(call(P->sorted), P->sorted_cq_own, max_len, gs, ctx->sm_count, &variant); break;
             case G_SPECTRAL: {
                 SpectralArgs A = call(P->spectral);
                 A.twiddle = ctx->d_tw; A.tw_n = ctx->tw_n;
                 e = launch_spectral(A, max_len, gs, ctx->sm_count, &variant);
                 break;
             }
-            case G_LA: e = launch_la(call(P->la), max_len, gs, ctx->sm_count, &variant); break;
+            case G_LA: e = launch_la(call(P->la), P->la_tstat, max_len, gs, ctx->sm_count, &variant); break;
             case G_ENTROPY: e = launch_entropy(call(P->entropy), max_len, gs, ctx->sm_count, &variant); break;
             case G_SEQ: e = launch_seq(call(P->seq), max_len, gs, ctx->sm_count, &variant); break;
             case G_PEAKS: {

@@ -63,6 +63,79 @@ __device__ __forceinline__ int wmini(int v) { return __reduce_min_sync(FULL, v);
 // count of lanes (x tiles) where pred holds; every lane must call with its own predicate
 __device__ __forceinline__ int wcount(bool pred) { return __popc(__ballot_sync(FULL, pred)); }
 
+// ---------------------------------------------------------------- numpy reducers (f_agg), one warp
+// np.<f_agg> of the values x of the items i < m that get(i, x) selects (np_stats, then np_finish); f_agg is a TSFX_AGG_*
+// code, with TSFX_AGG_NANSKIP the np.nan* variant.  Plain reducers propagate NaN; on no
+// value (all NaN under NANSKIP, or nothing selected) sum gives 0, prod 1 and the others NaN.  var / std use ddof 0.  The
+// median selects its two middle values by bisection over order-preserving 64-bit keys: 64 counting sweeps, no storage.
+__device__ __forceinline__ unsigned long long np_key(double x) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
+    return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+__device__ __forceinline__ double np_unkey(unsigned long long k) {
+    return __longlong_as_double((long long)((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k));
+}
+// one sweep: count, NaN count, sum, product, max and min of the selected values (NaN apart)
+struct NpStats { int c, nans; double s, p, mx, mn; };
+template <typename F>
+__device__ __forceinline__ NpStats np_stats(F get, int m, int lane) {
+    NpStats S = {0, 0, 0.0, 1.0, -dinf(), dinf()};
+    for (int i = lane; i < m; i += 32) {
+        double x;
+        if (!get(i, x)) continue;
+        if (x != x) { ++S.nans; continue; }
+        ++S.c; S.s += x; S.p *= x; S.mx = fmax(S.mx, x); S.mn = fmin(S.mn, x);
+    }
+    S.c = wsumi(S.c); S.nans = wsumi(S.nans); S.s = wsum(S.s); S.mx = wmax(S.mx); S.mn = wmin(S.mn);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) S.p *= __shfl_xor_sync(FULL, S.p, o);
+    return S;
+}
+// the reducer from the sweep's statistics; var / std and the median sweep the values again
+template <typename F>
+__device__ __forceinline__ double np_finish(const NpStats& S, F get, int m, int f_agg, int lane) {
+    const bool skip = (f_agg & TSFX_AGG_NANSKIP) != 0;
+    const int op = f_agg & ~TSFX_AGG_NANSKIP;
+    const int c = S.c;
+    if (S.nans > 0 && !skip) return dnan();
+    if (op == TSFX_AGG_SUM) return S.s;
+    if (op == TSFX_AGG_PROD) return S.p;
+    if (c == 0) return dnan();
+    if (op == TSFX_AGG_MAX) return S.mx;
+    if (op == TSFX_AGG_MIN) return S.mn;
+    if (op == TSFX_AGG_PTP) return S.mx - S.mn;
+    const double mu = S.s / (double)c;
+    if (op == TSFX_AGG_MEAN) return mu;
+    if (op == TSFX_AGG_VAR || op == TSFX_AGG_STD) {
+        double q = 0.0;
+        for (int i = lane; i < m; i += 32) {
+            double x;
+            if (get(i, x) && x == x) { const double d = x - mu; q = fma(d, d, q); }
+        }
+        const double v = wsum(q) / (double)c;
+        return op == TSFX_AGG_STD ? sqrt(v) : v;
+    }
+    // TSFX_AGG_MEDIAN: the smallest key with more than k values at or below it is the k-th smallest value
+    double mid2[2];
+#pragma unroll 1
+    for (int h = 0; h < 2; ++h) {
+        const int k = h ? c / 2 : (c - 1) / 2;
+        unsigned long long lo = 0ull, hi = ~0ull;
+#pragma unroll 1
+        while (lo < hi) {
+            const unsigned long long md = lo + ((hi - lo) >> 1);
+            int at = 0;
+            for (int i = lane; i < m; i += 32) {
+                double x;
+                if (get(i, x) && x == x && np_key(x) <= md) ++at;
+            }
+            if (wsumi(at) > k) hi = md; else lo = md + 1;
+        }
+        mid2[h] = np_unkey(lo);
+    }
+    return 0.5 * (mid2[0] + mid2[1]);
+}
+
 // ---------------------------------------------------------------- per-warp working region
 // Normally a slice of the CTA's dynamic shared memory.  Series too long for that (bytes_per_warp > 227 KB) run
 // with the same carve-up in a global-memory scratch buffer (L2-resident; slower, but every length works).

@@ -183,7 +183,9 @@ struct BasicArgs : GroupArgs {
     int pacf_off;        // offset (doubles) of the pacf staging area inside lagS
     const double* dec;   // device table d*10^k, k = TSFX_DEC_MIN..TSFX_DEC_MAX, 9 per decade
 };
-cudaError_t launch_basic(const BasicArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
+// vocab: the plan has a column basic_vocabulary (k_basic.cu) finishes: agg_autocorrelation with a reducer other than
+// mean / median / var / std, or linregress attr intercept_stderr
+cudaError_t launch_basic(const BasicArgs& A, bool vocab, int max_len, cudaStream_t st, int sm_count, const char** variant);
 bool basic_finisher_calc(int calc);
 bool sorted_finisher_calc(int calc);    // same for the SORTED group     // host: is this calculator evaluated by the lane-parallel finisher stage?
 
@@ -205,7 +207,8 @@ struct SortedArgs : GroupArgs {
     int nfin, ncq;       // leading O(1) descriptors (lane-parallel); distinct change_quantiles corridors
     const double2* cq;   // device: (ql, qh) of every distinct corridor, in descriptor order
 };
-cudaError_t launch_sorted(const SortedArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
+// cq_own: some change_quantiles column's reducer is not mean / var / std (cq_own_passes, k_sorted.cu)
+cudaError_t launch_sorted(const SortedArgs& A, bool cq_own, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct SpectralArgs : GroupArgs {
     int npad, nspec, bytes_per_warp;
@@ -223,7 +226,8 @@ cudaError_t launch_spectral(const SpectralArgs& A, int max_len, cudaStream_t st,
 struct LaArgs : GroupArgs {
     int npad, max_ar_k, bytes_per_warp;    // max_ar_k: the plan's largest ar_coefficient order k
 };
-cudaError_t launch_la(const LaArgs& A, int max_len, cudaStream_t st, int sm_count, const char** variant);
+// tstat: some augmented_dickey_fuller column uses autolag "t-stat"
+cudaError_t launch_la(const LaArgs& A, bool tstat, int max_len, cudaStream_t st, int sm_count, const char** variant);
 
 struct EntropyArgs : GroupArgs {
     int xpad;                  // tile kernel: padded sample count

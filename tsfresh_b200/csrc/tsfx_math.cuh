@@ -123,6 +123,12 @@ TSFX_HD double m_linreg_pick(const LinReg& R, int attr) {
     }
 }
 
+// intercept_stderr of the same fit (scipy: slope_stderr * sqrt(ssxm + xmean^2)); the callers pick it before
+// m_linreg_pick, whose LinReg does not carry the regressor's moments
+TSFX_HD double m_intercept_stderr(double slope_stderr, double xmean, double ssxm) {
+    return slope_stderr * sqrt(ssxm + xmean * xmean);
+}
+
 // ------------------------------------------------------------------ dense SPD solves (row-major, lda)
 // In-place lower Cholesky of the leading n x n block.  Returns false on a non-positive pivot.
 TSFX_HD bool m_cholesky(double* A, int n, int lda) {

@@ -29,11 +29,17 @@ CALC = _parse_calc_enum()
 CALC_NAME = {v: k for k, v in CALC.items()}
 
 AGG = {"mean": 0, "median": 1, "var": 2, "std": 3, "max": 4, "min": 5}
+AGG_NANSKIP = 16            # TSFX_AGG_NANSKIP: the np.nan* variant of a reducer
+# numpy functions agg_autocorrelation and change_quantiles accept as f_agg (the reference calls getattr(np, f_agg))
+AGG_NUMPY = dict(AGG, amax=4, amin=5, ptp=6, sum=7, prod=8, average=0,
+                 **{"nan" + k: v | AGG_NANSKIP for k, v in (("mean", 0), ("median", 1), ("var", 2), ("std", 3), ("max", 4),
+                                                             ("min", 5), ("sum", 7), ("prod", 8))})
+AGG_RAISES_ON_EMPTY = ("max", "amax", "min", "amin", "ptp", "nanmax", "nanmin")
 FFT_ATTR = {"real": 0, "imag": 1, "abs": 2, "angle": 3}
 SPEC_ATTR = {"centroid": 0, "variance": 1, "skew": 2, "kurtosis": 3}
-LR_ATTR = {"pvalue": 0, "rvalue": 1, "intercept": 2, "slope": 3, "stderr": 4}
+LR_ATTR = {"pvalue": 0, "rvalue": 1, "intercept": 2, "slope": 3, "stderr": 4, "intercept_stderr": 5}
 ADF_ATTR = {"teststat": 0, "pvalue": 1, "usedlag": 2}
-AUTOLAG = {"AIC": 0, "BIC": 1, None: 2}
+AUTOLAG = {"aic": 0, "bic": 1, None: 2, "t-stat": 3}     # statsmodels lower-cases the name
 
 
 class tsfx_feature_desc(ctypes.Structure):
@@ -88,9 +94,16 @@ MAX_LZ_BINS = 65535         # lempel_ziv_complexity: 16-bit symbols, and the all
 # ------------------------------------------------------------------------------------------------
 # simple calculators: name -> (required keys, lambda(param) -> dict(attr,i0,i1,i2,p0,p1))
 def _s_agg(name, f_agg, allowed):
-    if f_agg not in allowed:
+    if not isinstance(f_agg, str) or f_agg not in allowed:
         _unsupported(name, "f_agg=%r" % (f_agg,))
-    return AGG[f_agg]
+    return AGG_NUMPY[f_agg]
+
+
+def _lr_attr(name, attr):
+    """linregress attribute code; the reference's getattr(LinregressResult, attr) raises AttributeError for any other"""
+    if not isinstance(attr, str) or attr not in LR_ATTR:
+        raise AttributeError("%s: 'LinregressResult' object has no attribute %r" % (name, attr))
+    return LR_ATTR[attr]
 
 
 _SIMPLE_NO_PARAM = {
@@ -129,7 +142,7 @@ def _simple_with_params(name, p):
         _need(name, p, ["ql", "qh", "isabs", "f_agg"])
         f["p0"], f["p1"] = float(p["ql"]), float(p["qh"])
         f["i0"] = 1 if p["isabs"] else 0
-        f["attr"] = _s_agg(name, p["f_agg"], ("mean", "var", "std", "median"))
+        f["attr"] = _s_agg(name, p["f_agg"], AGG_NUMPY)
     elif name == "mean_n_absolute_max":
         _need(name, p, ["number_of_maxima"]); f["i0"] = _int(name, "number_of_maxima", p["number_of_maxima"], 1)
     elif name == "approximate_entropy":
@@ -234,10 +247,12 @@ class Plan:
 
     def _c_agg_autocorrelation(self, plist, b):  # :432
         for p in plist:
-            a = _s_agg("agg_autocorrelation", p["f_agg"], ("mean", "median", "var", "std"))
+            a = _s_agg("agg_autocorrelation", p["f_agg"], AGG_NUMPY)
+            maxlag = _int("agg_autocorrelation", "maxlag", p["maxlag"], 0, MAX_LAG)
+            if maxlag == 0 and p["f_agg"] in AGG_RAISES_ON_EMPTY:
+                getattr(np, p["f_agg"])(np.zeros(0))    # numpy's ValueError: the reference's a[:0] is empty for every series
             yield ('f_agg_"%s"__maxlag_%s' % (p["f_agg"], p["maxlag"]),
-                   dict(b, calc=CALC["TSFX_AGG_AUTOCORRELATION"], attr=a,
-                        i0=_int("agg_autocorrelation", "maxlag", p["maxlag"], 0, MAX_LAG)))
+                   dict(b, calc=CALC["TSFX_AGG_AUTOCORRELATION"], attr=a, i0=maxlag))
 
     def _c_partial_autocorrelation(self, plist, b):  # :495
         top = max(_int("partial_autocorrelation", "lag", p["lag"], 0, MAX_LAG) for p in plist)
@@ -247,10 +262,14 @@ class Plan:
     def _c_augmented_dickey_fuller(self, plist, b):  # :534
         for p in plist:
             al = p.get("autolag", "AIC")
-            if al not in AUTOLAG:
+            if al is not None and not isinstance(al, str):
                 _unsupported("augmented_dickey_fuller", "autolag=%r" % (al,))
-            yield ('attr_"%s"__autolag_"%s"' % (p["attr"], al),
-                   dict(b, calc=CALC["TSFX_AUGMENTED_DICKEY_FULLER"], attr=ADF_ATTR.get(p["attr"], 3), i0=AUTOLAG[al]))
+            key = al.lower() if isinstance(al, str) else al
+            suffix = 'attr_"%s"__autolag_"%s"' % (p["attr"], al)
+            if key not in AUTOLAG:      # adfuller raises ValueError, which the reference turns into NaN (:520-526)
+                yield suffix, dict(b, calc=CALC["TSFX_CONST_NAN"])
+                continue
+            yield suffix, dict(b, calc=CALC["TSFX_AUGMENTED_DICKEY_FULLER"], attr=ADF_ATTR.get(p["attr"], 3), i0=AUTOLAG[key])
 
     def _c_fft_coefficient(self, plist, b):  # :1088-1118
         assert min(p["coeff"] for p in plist) >= 0, "Coefficients must be positive or zero."
@@ -272,9 +291,7 @@ class Plan:
 
     def _c_linear_trend(self, plist, b):  # :1364
         for p in plist:
-            if p["attr"] not in LR_ATTR:
-                _unsupported("linear_trend", "attr=%r" % (p["attr"],))
-            yield 'attr_"%s"' % (p["attr"],), dict(b, calc=CALC["TSFX_LINEAR_TREND"], attr=LR_ATTR[p["attr"]])
+            yield 'attr_"%s"' % (p["attr"],), dict(b, calc=CALC["TSFX_LINEAR_TREND"], attr=_lr_attr("linear_trend", p["attr"]))
 
     def _c_cwt_coefficients(self, plist, b):  # :1396-1412
         for p in plist:
@@ -308,11 +325,10 @@ class Plan:
 
     def _c_agg_linear_trend(self, plist, b):  # :2198-2220
         for p in plist:
-            if p["attr"] not in LR_ATTR:
-                _unsupported("agg_linear_trend", "attr=%r" % (p["attr"],))
+            attr = _lr_attr("agg_linear_trend", p["attr"])
             fa = _s_agg("agg_linear_trend", p["f_agg"], ("max", "min", "mean", "var", "std", "median"))
             yield ('attr_"%s"__chunk_len_%s__f_agg_"%s"' % (p["attr"], p["chunk_len"], p["f_agg"]),
-                   dict(b, calc=CALC["TSFX_AGG_LINEAR_TREND"], attr=LR_ATTR[p["attr"]],
+                   dict(b, calc=CALC["TSFX_AGG_LINEAR_TREND"], attr=attr,
                         i0=_int("agg_linear_trend", "chunk_len", p["chunk_len"], 1), i1=fa))
 
     def _c_energy_ratio_by_chunks(self, plist, b):  # :2251-2265
@@ -327,9 +343,8 @@ class Plan:
     def _c_linear_trend_timewise(self, plist, b):  # :2302-2305 (only reached with a DatetimeIndex)
         self.needs_times = True
         for p in plist:
-            if p["attr"] not in LR_ATTR:
-                _unsupported("linear_trend_timewise", "attr=%r" % (p["attr"],))
-            yield 'attr_"%s"' % p["attr"], dict(b, calc=CALC["TSFX_LINEAR_TREND_TIMEWISE"], attr=LR_ATTR[p["attr"]])
+            yield 'attr_"%s"' % p["attr"], dict(b, calc=CALC["TSFX_LINEAR_TREND_TIMEWISE"],
+                                                attr=_lr_attr("linear_trend_timewise", p["attr"]))
 
     def _c_query_similarity_count(self, plist, b):  # :2505-2519
         for p in plist:
