@@ -52,10 +52,16 @@ extern "C" {
 #define TSFX_FLAG_TIMING 2u      /* record CUDA events around every kernel group (tsfx_get_timings) */
 #define TSFX_FLAG_NO_NAN_CHECK 4u /* host-pointer extract calls scan the values for NaN and return TSFX_E_NAN (the reference
                                   * raises ValueError, data.py:148-167); this flag skips the scan.  Device-pointer calls
-                                  * (asynchronous) never scan. */
+                                  * (asynchronous) scan only with TSFX_FLAG_CHECK_DEVICE_INPUT. */
 #define TSFX_FLAG_IMPUTE 8u      /* extract calls: impute the feature matrix on the device before it is returned
                                   * (extract_features(impute_function=impute), extraction.py:179-181, 286-287) */
 #define TSFX_FLAG_ALL_MEDIANS 16u /* tsfx_impute: compute every column's median, not only those a NaN needs */
+#define TSFX_FLAG_CHECK_DEVICE_INPUT 32u /* with TSFX_FLAG_DEVICE_PTRS, tsfx_extract_csr / tsfx_extract_dense first make ONE
+                                  * pass over the input on the device and synchronise the stream once to read its result:
+                                  * the longest series (tsfx_set_max_len_hint is ignored), every (begin, len) view inside
+                                  * [0, n_values) with len >= 1 (else TSFX_E_INVALID), and no NaN among the values the
+                                  * series cover (else TSFX_E_NAN).  No kernel group runs on input that fails the pass,
+                                  * so tsfx_last_launch_count is 0 after such an error. */
 
 /* tsfx_impute modes (tsfresh/utilities/dataframe_functions.py) */
 #define TSFX_IMPUTE_RANGE 0      /* impute :49-78: +inf -> max, -inf -> min, NaN -> median of the finite values */
@@ -177,6 +183,12 @@ typedef struct tsfx_plan tsfx_plan;
  * a cudaStream_t the caller owns (e.g. torch's current stream) so caller-side CUDA events see the work. */
 int tsfx_ctx_create(int device, void* cuda_stream, tsfx_ctx** out);
 void tsfx_ctx_destroy(tsfx_ctx* ctx);
+/* Rebinds the stream the context's calls are enqueued on, so one context (and its working memory) serves whichever
+ * stream the caller is on.  cuda_stream is a stream of the context's device, or NULL for the stream the context was
+ * created with; pass cudaStreamLegacy ((void*)1) for the legacy default stream.  The new stream first waits for
+ * everything already enqueued on the old one (the calls reuse the context's scratch); the side streams, copy streams
+ * and timing events of later calls fork from and join to the new stream.  Does not block the host. */
+int tsfx_ctx_set_stream(tsfx_ctx* ctx, void* cuda_stream);
 const char* tsfx_last_error(const tsfx_ctx* ctx); /* ctx may be NULL: last creation error */
 int tsfx_sync(tsfx_ctx* ctx);
 int tsfx_version(void);
@@ -201,6 +213,12 @@ int tsfx_extract_csr(tsfx_ctx* ctx, const tsfx_plan* plan, const float* values, 
  * rolled windows) passes it here and the calls stay asynchronous.  The bound must hold for every series of the
  * following device-pointer tsfx_extract_csr calls; 0 removes the hint. */
 int tsfx_set_max_len_hint(tsfx_ctx* ctx, int32_t max_len);
+
+/* Row stride (in doubles) of `out` for the following device-pointer tsfx_extract_csr / tsfx_extract_dense calls, so
+ * that several plans (one per kind) fill column blocks of one matrix: row s of a call goes to out + s * ld.  ld must be
+ * >= the plan's n_cols (else the call returns TSFX_E_INVALID); 0 removes the setting (ld = n_cols).  A strided call
+ * cannot take TSFX_FLAG_IMPUTE (imputation needs every column of the matrix: impute it afterwards with tsfx_impute). */
+int tsfx_set_out_ld(tsfx_ctx* ctx, int32_t ld);
 
 /* Row timestamps for linear_trend_timewise (feature_calculators.py:2274-2306: the regressor is the series' DatetimeIndex,
  * hours since its first row).  row_time_ns[i] is the timestamp (int64 nanoseconds) of row i of the `values` array of the

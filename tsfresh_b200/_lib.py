@@ -17,6 +17,8 @@ FLAG_TIMING = 2
 FLAG_NO_NAN_CHECK = 4
 FLAG_IMPUTE = 8
 FLAG_ALL_MEDIANS = 16
+FLAG_CHECK_DEVICE_INPUT = 32
+STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy default stream for tsfx_ctx_set_stream
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
 
@@ -29,7 +31,8 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_plan_create", "tsfx_plan_destroy", "tsfx_extract_csr", "tsfx_extract_dense",
            "tsfx_extract_long", "tsfx_build_csr", "tsfx_roll_windows", "tsfx_get_timings",
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
-           "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression"]
+           "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
+           "tsfx_ctx_set_stream", "tsfx_set_out_ld"]
 
 
 def load():
@@ -72,6 +75,8 @@ def load():
         lib.tsfx_set_peer_outputs.argtypes = [vp, vp, i32, i32, ctypes.c_uint64, i32]
         lib.tsfx_peer_flush.argtypes = [vp]
         lib.tsfx_set_max_len_hint.argtypes = [vp, i32]
+        lib.tsfx_ctx_set_stream.argtypes = [vp, vp]
+        lib.tsfx_set_out_ld.argtypes = [vp, i32]
         lib.tsfx_set_row_times.argtypes = [vp, vp, i64, u32]
         lib.tsfx_select_classification.argtypes = [vp, vp, i64, i32, vp, i32, vp, u32]
         lib.tsfx_select_regression.argtypes = [vp, vp, i64, i32, vp, vp, u32]
@@ -136,6 +141,15 @@ class Context:
 
     def sync(self):
         self.check(self.lib.tsfx_sync(self.h), "tsfx_sync")
+
+    def set_stream(self, stream):
+        """tsfx_ctx_set_stream: enqueue the following calls on `stream` (a cudaStream_t as int; None: the stream the
+        context was created with; STREAM_LEGACY: the legacy default stream)."""
+        self.check(self.lib.tsfx_ctx_set_stream(self.h, ctypes.c_void_p(stream) if stream else None), "tsfx_ctx_set_stream")
+
+    def set_out_ld(self, ld):
+        """tsfx_set_out_ld: row stride (doubles) of `out` of the following device-pointer calls; 0 = the plan's n_cols"""
+        self.check(self.lib.tsfx_set_out_ld(self.h, int(ld)), "tsfx_set_out_ld")
 
     def timings(self):
         ms = (ctypes.c_float * 16)()
@@ -330,6 +344,22 @@ class DevicePlan:
         rc = self.ctx.lib.tsfx_extract_dense(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_series, length,
                                              ctypes.c_void_p(out_ptr), flags)
         self.ctx.check(rc, "tsfx_extract_dense")
+
+    def extract_dense_checked(self, values_ptr, n_series, length, out_ptr):
+        """tsfx_extract_dense on device pointers after the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT)"""
+        flags = FLAG_DEVICE_PTRS | FLAG_CHECK_DEVICE_INPUT
+        rc = self.ctx.lib.tsfx_extract_dense(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_series, length,
+                                             ctypes.c_void_p(out_ptr), flags)
+        self.ctx.check(rc, "tsfx_extract_dense")
+
+    def extract_csr_checked(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr):
+        """tsfx_extract_csr on device pointers after the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT): the views are
+        validated and the longest one measured on the device, whatever tsfx_set_max_len_hint holds"""
+        flags = FLAG_DEVICE_PTRS | FLAG_CHECK_DEVICE_INPUT
+        rc = self.ctx.lib.tsfx_extract_csr(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_values,
+                                           ctypes.c_void_p(begin_ptr), ctypes.c_void_p(len_ptr), n_series,
+                                           ctypes.c_void_p(out_ptr), flags)
+        self.ctx.check(rc, "tsfx_extract_csr")
 
     def extract_csr_device(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr, timing=False, max_len=0):
         """max_len: upper bound of the series lengths if the caller knows one (keeps the call asynchronous)"""

@@ -357,10 +357,12 @@ __device__ __forceinline__ LinSums linreg_sums(const double* y, int k, int lane)
     return L;
 }
 
-// leading decimal digit of |v| (shortest-repr digit == true digit for float32-origin values; 0 -> 0)
+// leading decimal digit of |v| (shortest-repr digit == true digit for float32-origin values; 0 -> 0).  The reference
+// takes np.nan_to_num first: +-inf becomes +-DBL_MAX (1.79e308), digit 1; ilogb(inf) would index far past the table.
 __device__ __forceinline__ int leading_digit(float f, const double* dec) {
     float a = fabsf(f);
     if (a == 0.f) return 0;
+    if (isinf(a)) return 1;
     double v = (double)a;
     int e = ilogb(v);
     int k = (int)floor((double)e * 0.30102999566398120);

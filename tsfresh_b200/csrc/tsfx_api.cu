@@ -231,8 +231,10 @@ static const char* kGroupNames[G_EVENTS] = {"basic", "sorted", "spectral", "la",
 
 struct tsfx_ctx {
     int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
+    cudaStream_t stream = nullptr;        // where calls are enqueued (tsfx_ctx_set_stream)
+    cudaStream_t home_stream = nullptr;   // the stream of tsfx_ctx_create
+    bool own_stream = false;              // home_stream was created by the library
+    cudaEvent_t ev_rebind = nullptr;
     int sm_count = 132;                   // replaced by the device's multiProcessorCount in tsfx_create
     std::string err;
     DevBuf values, begin, len, out, misc, stage;
@@ -258,6 +260,7 @@ struct tsfx_ctx {
     const int64_t* times_ptr = nullptr;
     int64_t times_rows = -1;
     int max_len_hint = 0;        // tsfx_set_max_len_hint: longest series of the coming device-pointer CSR calls
+    int out_ld = 0;              // tsfx_set_out_ld: row stride of `out` of the coming device-pointer calls (0: n_cols)
     HostPool pool;
     Stager stager;
     // multi-GPU result placement (tsfx_set_peer_outputs): peers' mapped result matrices
@@ -378,6 +381,8 @@ extern "C" int tsfx_ctx_create(int device, void* cuda_stream, tsfx_ctx** out) {
     ctx->sm_count = prop.multiProcessorCount;
     if (cuda_stream) { ctx->stream = (cudaStream_t)cuda_stream; ctx->own_stream = false; }
     else { CKC(cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking)); ctx->own_stream = true; }
+    ctx->home_stream = ctx->stream;
+    CKC(cudaEventCreateWithFlags(&ctx->ev_rebind, cudaEventDisableTiming));
     for (int g = 0; g < G_EVENTS; ++g) { CKC(cudaEventCreate(&ctx->ev[g][0])); CKC(cudaEventCreate(&ctx->ev[g][1])); }
     CKC(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
     CKC(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
@@ -407,6 +412,7 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     if (!ctx) return;
     cudaSetDevice(ctx->device);
     cudaStreamSynchronize(ctx->stream);
+    cudaStreamSynchronize(ctx->home_stream);
     ctx->values.release(); ctx->begin.release(); ctx->len.release(); ctx->out.release(); ctx->misc.release(); ctx->stage.release();
     ctx->times.release(); ctx->times_sorted.release(); ctx->kvals.release(); ctx->kvals_sorted.release();
     ctx->csr.release();
@@ -426,8 +432,21 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     if (ctx->s_in) cudaStreamDestroy(ctx->s_in);
     if (ctx->s_out) cudaStreamDestroy(ctx->s_out);
     for (int i = 0; i < 2; ++i) { if (ctx->ev_in[i]) cudaEventDestroy(ctx->ev_in[i]); if (ctx->ev_done[i]) cudaEventDestroy(ctx->ev_done[i]); }
-    if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
+    if (ctx->ev_rebind) cudaEventDestroy(ctx->ev_rebind);
+    if (ctx->own_stream && ctx->home_stream) cudaStreamDestroy(ctx->home_stream);
     delete ctx;
+}
+
+extern "C" int tsfx_ctx_set_stream(tsfx_ctx* ctx, void* cuda_stream) {
+    if (!ctx) return TSFX_E_INVALID;
+    cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : ctx->home_stream;
+    if (next == ctx->stream) return TSFX_OK;
+    CK(cudaSetDevice(ctx->device));
+    // the next calls reuse the scratch (and twiddle / Ricker tables) the work on the old stream may still be using
+    CK(cudaEventRecord(ctx->ev_rebind, ctx->stream));
+    CK(cudaStreamWaitEvent(next, ctx->ev_rebind, 0));
+    ctx->stream = next;
+    return TSFX_OK;
 }
 
 extern "C" int tsfx_sync(tsfx_ctx* ctx) {
@@ -885,6 +904,39 @@ static int check_args(tsfx_ctx* ctx, const tsfx_plan* plan, const void* values, 
     return TSFX_OK;
 }
 
+// TSFX_FLAG_CHECK_DEVICE_INPUT: one pass over the caller's device input (views when begin != nullptr, else n_values
+// values of a dense batch) and one synchronisation, before any kernel group can see the input
+static int check_device_input(tsfx_ctx* ctx, const float* values, int64_t n_values, const int64_t* begin, const int32_t* len,
+                              int64_t n_series, int* max_len) {
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    CsrWorkspace& W = ctx->csr;
+    CK(W.init_info());
+    CK(cudaMemsetAsync(W.d_info, 0, sizeof(CsrInfo), ctx->stream));
+    if (begin) csr_check_views(W, values, n_values, begin, len, n_series, ctx->stream);
+    else csr_check_nan(W, values, n_values, ctx->stream);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(W.h_info, W.d_info, sizeof(CsrInfo), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    const CsrInfo& I = *W.h_info;
+    if (I.bad_view_rev)
+        return fail(ctx, TSFX_E_INVALID, "series " + std::to_string(n_series - (int64_t)I.bad_view_rev) +
+                                             " has an invalid (begin, len): len < 1, begin < 0 or begin + len > n_values");
+    if (I.has_nan) return nan_error(ctx);
+    if (begin) *max_len = I.max_len;
+    return TSFX_OK;
+}
+
+// row stride of a device-pointer call's `out` (tsfx_set_out_ld)
+static int device_out_ld(tsfx_ctx* ctx, const tsfx_plan* plan, uint32_t flags, int* ld) {
+    *ld = ctx->out_ld > 0 ? ctx->out_ld : plan->ncols;
+    if (*ld < plan->ncols)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_set_out_ld: row stride " + std::to_string(*ld) + " < " + std::to_string(plan->ncols) + " columns");
+    if (*ld != plan->ncols && (flags & TSFX_FLAG_IMPUTE))
+        return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_IMPUTE needs a contiguous result matrix (tsfx_set_out_ld)");
+    return TSFX_OK;
+}
+
 extern "C" int tsfx_extract_csr(tsfx_ctx* ctx, const tsfx_plan* plan, const float* values, int64_t n_values,
                                 const int64_t* begin, const int32_t* len, int64_t n_series, double* out,
                                 uint32_t flags) {
@@ -901,12 +953,18 @@ extern "C" int tsfx_extract_csr(tsfx_ctx* ctx, const tsfx_plan* plan, const floa
     int max_len = 0;
     if (flags & TSFX_FLAG_DEVICE_PTRS) {
         R.values = values; R.begin = begin; R.len = len;
-        if (ctx->max_len_hint > 0) max_len = ctx->max_len_hint;       // stays asynchronous
+        int ld = 0;
+        rc = device_out_ld(ctx, plan, flags, &ld);
+        if (rc) return rc;
+        if (flags & TSFX_FLAG_CHECK_DEVICE_INPUT) {
+            rc = check_device_input(ctx, values, n_values, begin, len, n_series, &max_len);
+            if (rc) return rc;
+        } else if (ctx->max_len_hint > 0) max_len = ctx->max_len_hint;       // stays asynchronous
         else {
             int rc2 = csr_max_len(ctx->csr, len, n_series, ctx->stream, &max_len);
             if (rc2) return fail(ctx, TSFX_E_CUDA, "max-length reduction failed");
         }
-        rc = run_groups(ctx, plan, R, max_len, out, flags);
+        rc = run_groups(ctx, plan, R, max_len, out, flags, ld);
         if (!rc && (flags & TSFX_FLAG_IMPUTE)) rc = impute_after_extract(ctx, out, n_series, plan->ncols);
         return rc;
     }
@@ -955,7 +1013,15 @@ extern "C" int tsfx_extract_dense(tsfx_ctx* ctx, const tsfx_plan* plan, const fl
     R.times = all_times;
     if (flags & TSFX_FLAG_DEVICE_PTRS) {
         R.values = values;
-        rc = run_groups(ctx, plan, R, len, out, flags);
+        int ld = 0;
+        rc = device_out_ld(ctx, plan, flags, &ld);
+        if (rc) return rc;
+        if (flags & TSFX_FLAG_CHECK_DEVICE_INPUT) {
+            int max_len = len;
+            rc = check_device_input(ctx, values, n_series * (int64_t)len, nullptr, nullptr, n_series, &max_len);
+            if (rc) return rc;
+        }
+        rc = run_groups(ctx, plan, R, len, out, flags, ld);
         if (!rc && (flags & TSFX_FLAG_IMPUTE)) rc = impute_after_extract(ctx, out, n_series, plan->ncols);
         return rc;
     }
@@ -1561,6 +1627,12 @@ extern "C" int tsfx_set_peer_outputs(tsfx_ctx* ctx, const uint64_t* peer_out, in
 extern "C" int tsfx_set_max_len_hint(tsfx_ctx* ctx, int32_t max_len) {
     if (!ctx || max_len < 0) return TSFX_E_INVALID;
     ctx->max_len_hint = max_len;
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_set_out_ld(tsfx_ctx* ctx, int32_t ld) {
+    if (!ctx || ld < 0) return TSFX_E_INVALID;
+    ctx->out_ld = ld;
     return TSFX_OK;
 }
 

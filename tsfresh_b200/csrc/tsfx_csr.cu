@@ -72,6 +72,28 @@ __global__ void k_check_nan(const float* __restrict__ values, int64_t n, CsrInfo
     if (__any_sync(0xffffffffu, nan) && (threadIdx.x & 31) == 0) atomicOr(&info->has_nan, 1);
 }
 
+// One warp per view: bounds and length of the view, then its samples (coalesced) for NaN.  Views may overlap (rolled
+// windows), so the scan follows the views rather than the value array: a NaN no series covers is not an error.
+__global__ void k_check_views(const float* __restrict__ values, int64_t n_values, const int64_t* __restrict__ begin,
+                              const int32_t* __restrict__ len, int64_t n_series, CsrInfo* info) {
+    const int lane = threadIdx.x & 31;
+    int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    int mx = 0, nan = 0;
+    for (; w < n_series; w += n_warps) {                  // warp-uniform
+        const int64_t b = begin[w];
+        const int32_t l = len[w];
+        if (l < 1 || b < 0 || b > n_values - l) {
+            if (lane == 0) atomicMax((unsigned long long*)&info->bad_view_rev, (unsigned long long)(n_series - w));
+            continue;
+        }
+        mx = max(mx, (int)l);
+        for (int32_t i = lane; i < l; i += 32) { const float v = values[b + i]; nan |= v != v; }
+    }
+    if (lane == 0 && mx > 0) atomicMax(&info->max_len, mx);
+    if (__any_sync(0xffffffffu, nan) && lane == 0) atomicOr(&info->has_nan, 1);
+}
+
 // len[s] = begin[s+1] - begin[s] (begin[n_series] = n_rows), longest series, row-block boundaries
 __global__ void k_len_info(const int64_t* __restrict__ begin, const int* __restrict__ d_nruns, int64_t n_rows,
                            int32_t* __restrict__ len, int64_t min_block, int max_blocks, CsrInfo* info) {
@@ -198,6 +220,12 @@ void csr_check_rows(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_key
 void csr_check_nan(CsrWorkspace& W, const float* d_values, int64_t n, cudaStream_t st) {
     if (n <= 0) return;
     k_check_nan<<<grid_for(n, 256), 256, 0, st>>>(d_values, n, W.d_info);
+}
+
+void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
+                     int64_t n_series, cudaStream_t st) {
+    if (n_series <= 0) return;
+    k_check_views<<<grid_for(n_series * 32, 256), 256, 0, st>>>(d_values, n_values, d_begin, d_len, n_series, W.d_info);
 }
 
 int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, const float* d_values,

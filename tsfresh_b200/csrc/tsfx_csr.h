@@ -26,6 +26,7 @@ struct CsrInfo {                  // written by the device, mirrored in pinned h
     int32_t pad;
     int64_t series_lo[TSFX_CSR_MAX_BLOCKS + 1];   // block b covers series [series_lo[b], series_lo[b+1])
     int64_t row_lo[TSFX_CSR_MAX_BLOCKS + 1];      //             and rows [row_lo[b], row_lo[b+1])
+    uint64_t bad_view_rev;        // csr_check_views: n_series - s for the first series s with an invalid view (0: none)
 };
 
 struct CsrWorkspace {
@@ -74,5 +75,11 @@ int csr_max_len(CsrWorkspace& W, const int32_t* d_len, int64_t n, cudaStream_t s
 
 // NaN scan of a device float array; result lands in d_info->has_nan (async)
 void csr_check_nan(CsrWorkspace& W, const float* d_values, int64_t n, cudaStream_t st);
+
+// Checked pass over caller-supplied device views (TSFX_FLAG_CHECK_DEVICE_INPUT), one launch: the longest series into
+// d_info->max_len, the first view with len < 1, begin < 0 or begin + len > n_values into d_info->bad_view_rev, and a NaN
+// among the values of the valid views into d_info->has_nan (async; d_info zeroed by the caller)
+void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
+                     int64_t n_series, cudaStream_t st);
 
 }  // namespace tsfx

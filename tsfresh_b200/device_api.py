@@ -1,0 +1,167 @@
+"""extract_features_device(): features of series that already live on the GPU, into a float64 matrix on the GPU.
+
+    X, columns = extract_features_device(values)                        # [N, L] or [N, L, K] channels-last
+    X, columns = extract_features_device(values, begin, length)         # CSR views: series s = values[begin[s]:+length[s]]
+
+No host copy of the series or of the result: the call enqueues its work on torch's current stream of the tensor's
+device and blocks the host once per kind, for the checked pass (include/tsfx.h, TSFX_FLAG_CHECK_DEVICE_INPUT) that
+measures the longest series and rejects invalid views and NaN values before any kernel group sees the input.
+Columns are named and ordered as `extract_features` names them for the equivalent wide frame (one value column per
+kind, no DatetimeIndex, so linear_trend_timewise is skipped); rows follow the input order.
+"""
+import numpy as np
+import pandas as pd
+
+from . import _lib
+from .dataframe_functions import impute, impute_dataframe_zero
+from .extraction import _check_colname, _device_plan, get_context
+from .plan import Plan
+from .settings import ComprehensiveFCParameters
+
+
+def _layout(values, begin, length, kinds):
+    """(number of series, kinds, CSR?) from the shapes and dtypes alone (no device needed)."""
+    import torch
+    if not isinstance(values, torch.Tensor):
+        raise TypeError("values must be a torch.Tensor, not %s" % type(values).__name__)
+    if values.dtype not in (torch.float32, torch.float64, torch.float16, torch.bfloat16):
+        raise TypeError("values must be float32, float64, float16 or bfloat16, not %s" % values.dtype)
+    csr = begin is not None or length is not None
+    if csr:
+        if begin is None or length is None:
+            raise ValueError("begin and length must be given together")
+        for name, t in (("begin", begin), ("length", length)):
+            if not isinstance(t, torch.Tensor):
+                raise TypeError("%s must be a torch.Tensor, not %s" % (name, type(t).__name__))
+            if t.ndim != 1:
+                raise ValueError("%s must be 1-D, got shape %s" % (name, tuple(t.shape)))
+        if begin.dtype != torch.int64:
+            raise TypeError("begin must be int64, not %s" % begin.dtype)
+        if length.dtype not in (torch.int32, torch.int64):
+            raise TypeError("length must be int32 or int64, not %s" % length.dtype)
+        if begin.shape[0] != length.shape[0]:
+            raise ValueError("begin has %d entries, length %d" % (begin.shape[0], length.shape[0]))
+        if values.ndim not in (1, 2):
+            raise ValueError("CSR values must be [R] or [R, K], got shape %s" % (tuple(values.shape),))
+        n, n_kinds = begin.shape[0], (1 if values.ndim == 1 else values.shape[1])
+    else:
+        if values.ndim not in (2, 3):
+            raise ValueError("dense values must be [N, L] or [N, L, K], got shape %s" % (tuple(values.shape),))
+        if values.shape[1] > 0x7fffffff:
+            raise ValueError("series of %d samples" % values.shape[1])
+        n, n_kinds = values.shape[0], (1 if values.ndim == 2 else values.shape[2])
+    if n_kinds < 1:
+        raise ValueError("values has no kind (K = 0)")
+    kinds = list(range(n_kinds)) if kinds is None else list(kinds)
+    if len(kinds) != n_kinds:
+        raise ValueError("%d kinds named for %d in values" % (len(kinds), n_kinds))
+    if len(set(map(str, kinds))) != len(kinds):
+        raise ValueError("kinds must have distinct names: %r" % (kinds,))
+    _check_colname(*kinds)
+    return n, kinds, csr
+
+
+def _plans(kinds, default_fc_parameters, kind_to_fc_parameters):
+    """One Plan per kind and the result's column names, as extract_features gives them for a wide frame."""
+    if default_fc_parameters is None and kind_to_fc_parameters is None:
+        default_fc_parameters = ComprehensiveFCParameters()
+    elif default_fc_parameters is None:
+        default_fc_parameters = {}
+    plans, columns = [], []
+    for kind in kinds:
+        fc = kind_to_fc_parameters[kind] if (kind_to_fc_parameters and kind in kind_to_fc_parameters) else default_fc_parameters
+        plan = Plan(fc, has_datetime_index=False)
+        plans.append(plan)
+        columns += [str(kind) + "__" + s for s in plan.suffixes]
+    return plans, columns
+
+
+def _check_out(out, n, width):
+    import torch
+    if not isinstance(out, torch.Tensor):
+        raise TypeError("out must be a torch.Tensor, not %s" % type(out).__name__)
+    if out.dtype != torch.float64:
+        raise TypeError("out must be float64, not %s" % out.dtype)
+    if tuple(out.shape) != (n, width):
+        raise ValueError("out has shape %s, the result is (%d, %d)" % (tuple(out.shape), n, width))
+    if n > 0 and width > 0 and ((width > 1 and out.stride(1) != 1) or out.stride(0) < width):
+        raise ValueError("out must have unit column stride and a row stride >= its width (got strides %s)" % (out.stride(),))
+
+
+def extract_features_device(values, begin=None, length=None, *, default_fc_parameters=None, kind_to_fc_parameters=None,
+                            kinds=None, impute_function=None, out=None):
+    """Extracts features from CUDA tensors into a CUDA tensor.
+
+    values: [N, L] or channels-last [N, L, K] (dense), or [R] / [R, K] with `begin` (int64) and `length` (int32 or
+    int64) CUDA tensors of N entries (series s is values[begin[s] : begin[s] + length[s]]; views may overlap).
+    float32 is read in place; float64, float16 and bfloat16 are rounded to float32 on the device.
+    default_fc_parameters / kind_to_fc_parameters: as extract_features; `kinds` names the K kinds (default 0 .. K-1).
+    impute_function: impute or impute_dataframe_zero impute on the device; any other callable gets a host DataFrame.
+    out: a float64 CUDA tensor [N, n_features] (or a column slice of a wider one) to fill instead of a new one.
+
+    Returns (X, columns): X float64 [N, n_features] on values' device, rows in input order.  Raises ValueError for
+    NaN values, invalid views and series longer than the plan allows, before any feature kernel runs."""
+    import torch
+    n, kinds, csr = _layout(values, begin, length, kinds)
+    plans, columns = _plans(kinds, default_fc_parameters, kind_to_fc_parameters)
+    width = len(columns)
+    if out is not None:
+        _check_out(out, n, width)
+    dev = values.device
+    if dev.type != "cuda":
+        raise ValueError("values must be a CUDA tensor, got one on %s" % dev)
+    for name, t in (("begin", begin), ("length", length), ("out", out)):
+        if t is not None and t.device != dev:
+            raise ValueError("%s is on %s, values on %s" % (name, t.device, dev))
+    mode = _lib.IMPUTE_RANGE if impute_function is impute else _lib.IMPUTE_ZERO if impute_function is impute_dataframe_zero else None
+    with torch.cuda.device(dev):
+        X = out if out is not None else torch.empty((n, width), dtype=torch.float64, device=dev)
+        if n == 0 or width == 0:
+            return X, columns
+        v = values if values.dtype == torch.float32 else values.to(torch.float32)
+        if csr:
+            b = begin.contiguous()
+            # int64 lengths beyond int32 become lengths the checked pass rejects, never wrapped-around valid ones
+            ln = length.contiguous() if length.dtype == torch.int32 else length.clamp(0, 0x7fffffff).to(torch.int32)
+        # device imputation needs the whole matrix contiguous: a strided `out` is filled through a contiguous one
+        target = X if (mode is None or X.stride(0) == width) else torch.empty((n, width), dtype=torch.float64, device=dev)
+        ctx = get_context(dev.index)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        scratch = None
+        with ctx.lock:
+            ctx.set_stream(stream or _lib.STREAM_LEGACY)
+            try:
+                ctx.set_out_ld(target.stride(0))
+                c0 = 0
+                for k, plan in enumerate(plans):
+                    if plan.n_cols == 0:
+                        continue
+                    if v.ndim == (2 if csr else 3):             # channels-last: this kind's values, contiguous
+                        scratch = torch.empty(v.shape[:-1], dtype=torch.float32, device=dev) if scratch is None else scratch
+                        col = scratch.copy_(v[..., k])
+                    else:
+                        col = v.contiguous()
+                    dp = _device_plan(ctx, plan)
+                    o = target.data_ptr() + c0 * 8
+                    try:
+                        if csr:
+                            dp.extract_csr_checked(col.data_ptr(), col.shape[0], b.data_ptr(), ln.data_ptr(), n, o)
+                        else:
+                            dp.extract_dense_checked(col.data_ptr(), n, col.shape[1], o)
+                    except ValueError as e:
+                        if "contains NaN" in str(e):        # data.py:148-167, the check every extraction path makes
+                            raise ValueError("Column must not contain NaN values: {}".format(kinds[k])) from None
+                        raise
+                    c0 += plan.n_cols
+                if mode is not None:
+                    ctx.impute_device(target.data_ptr(), n, width, mode)
+            finally:
+                ctx.set_out_ld(0)
+                ctx.set_stream(None)
+        if target is not X:
+            X.copy_(target)
+    if impute_function is not None and mode is None:
+        df = pd.DataFrame(X.cpu().numpy(), columns=columns)
+        impute_function(df)
+        X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
+    return X, columns
