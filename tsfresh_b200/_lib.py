@@ -238,6 +238,23 @@ class Context:
             self.check(rc, "tsfx_select_regression")
         return out[:f * 8].reshape(f, 8), out[f * 8:]
 
+    # device-pointer forms: X is a row-major float64 [n, f] matrix on the context's device, read in place on the
+    # context's stream; the targets stay host arrays.  Both calls end in a synchronisation of that stream.
+    def select_classification_device(self, X_ptr, n, f, y_codes, n_classes):
+        y = np.ascontiguousarray(y_codes, dtype=np.int32)
+        out = np.zeros((int(n_classes), f, 8), dtype=np.float64)
+        rc = self.lib.tsfx_select_classification(self.h, ctypes.c_void_p(X_ptr), n, f, _ptr(y), int(n_classes), _ptr(out),
+                                                 FLAG_DEVICE_PTRS)
+        self.check(rc, "tsfx_select_classification")
+        return out
+
+    def select_regression_device(self, X_ptr, n, f, y):
+        y = np.ascontiguousarray(y, dtype=np.float64)
+        out = np.zeros(f * 8 + 4, dtype=np.float64)
+        rc = self.lib.tsfx_select_regression(self.h, ctypes.c_void_p(X_ptr), n, f, _ptr(y), _ptr(out), FLAG_DEVICE_PTRS)
+        self.check(rc, "tsfx_select_regression")
+        return out[:f * 8].reshape(f, 8), out[f * 8:]
+
     def set_row_times(self, times_ns):
         """timestamps (int64 ns) of the rows of the NEXT extract call's values (linear_trend_timewise)"""
         t = np.ascontiguousarray(times_ns, dtype=np.int64)

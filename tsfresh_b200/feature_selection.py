@@ -21,7 +21,12 @@ REGRESSION targets (relevance.py:282-296) take tsfx_select_regression: real feat
 brought into (x, rank(y)) order by two stable device sorts, the discordant pairs are the strict inversions of the rank
 sequence (bottom-up merge, one kernel per level), tie sums come from the runs; binary features need the two-sample KS of
 the target between their two groups (one pass over the y-sorted rows).
+
+A feature matrix already on the GPU (extract_features_device) takes calculate_relevance_table_device /
+select_features_device: the library reads the CUDA tensor in place (TSFX_FLAG_DEVICE_PTRS) instead of staging a host
+copy, and the same host code turns the statistics into the table (_relevance_table).
 """
+import contextlib
 import math
 import warnings
 from functools import reduce
@@ -201,6 +206,22 @@ def calculate_relevance_table(X, y, ml_task="auto", multiclass=False, n_signific
     y = y.sort_index()
     X = X.sort_index()
     assert list(y.index) == list(X.index), "The index of X and y need to be the same"
+
+    def host_matrix():                   # the library copies it to the device (the context's selection scratch)
+        return np.ascontiguousarray(X.to_numpy(dtype=np.float64))
+    return _relevance_table(
+        list(X.columns), y, lambda codes, k: get_context(device).select_classification(host_matrix(), codes, k),
+        lambda yv: get_context(device).select_regression(host_matrix(), yv), ml_task, multiclass, n_significant,
+        show_warnings, test_for_binary_target_real_feature, fdr_level, hypotheses_independent)
+
+
+def _relevance_table(features, y, class_stats, regression_stats, ml_task, multiclass, n_significant, show_warnings,
+                     test_for_binary_target_real_feature, fdr_level, hypotheses_independent):
+    """relevance.py:172-322 from the sufficient statistics of the feature matrix, whose columns are `features` and
+    whose rows are the positions of the host Series `y`.  The matrix is only read through the two callables, called
+    after every argument check: class_stats(int32 codes, n_labels) -> [n_labels, n_features, 8] and
+    regression_stats(float64 y) -> ([n_features, 8], (ytie, y0, y1, n)), raising a ValueError that mentions NaN for a
+    NaN in the matrix."""
     if ml_task not in ["auto", "classification", "regression"]:
         raise ValueError("ml_task must be one of: 'auto', 'classification', 'regression'")
     elif ml_task == "auto":
@@ -214,20 +235,17 @@ def calculate_relevance_table(X, y, ml_task="auto", multiclass=False, n_signific
 
     with warnings.catch_warnings():
         warnings.simplefilter("default" if show_warnings else "ignore")
-        features = list(X.columns)
-        M = np.ascontiguousarray(X.to_numpy(dtype=np.float64))
-        ctx = get_context(device)
         try:
             if ml_task == "classification":
                 labels = list(y.unique())                # order of appearance, as the reference's loop (relevance.py:248)
                 codes = pd.Categorical(y, categories=labels).codes.astype(np.int32)
-                stats = ctx.select_classification(M, codes, len(labels))      # [n_labels, n_features, 8]
+                stats = class_stats(codes, len(labels))                   # [n_labels, n_features, 8]
                 type_col = stats[0, :, 0]
             else:
                 yv = np.ascontiguousarray(y.to_numpy(dtype=np.float64))
                 if np.isnan(yv).any():
                     raise ValueError("Target y contains NaN values")
-                rstats, ytail = ctx.select_regression(M, yv)                  # [n_features, 8], (ytie, y0, y1, n)
+                rstats, ytail = regression_stats(yv)                         # [n_features, 8], (ytie, y0, y1, n)
                 type_col = rstats[:, 0]
         except ValueError as e:
             if "NaN" in str(e) and "Target" not in str(e):
@@ -317,3 +335,122 @@ def select_features(X, y, test_for_binary_target_binary_feature=TEST_FOR_BINARY_
         hypotheses_independent=hypotheses_independent, device=device)
     relevant_features = relevance_table[relevance_table.relevant].feature
     return X.loc[:, relevant_features]
+
+
+# ------------------------------------------------------------------------------------------ feature matrices on the GPU
+def _device_args(X, y, columns):
+    """The checks of a CUDA matrix's arguments that need no device, and ONE host copy of the targets: a Series with a
+    RangeIndex, because X has no index and y is taken positionally (a Series is not aligned by its index).
+    That X is on a CUDA device is checked where the matrix is first read (_bound_context), after the checks of the
+    target and of ml_task / multiclass the DataFrame path makes, so those errors read the same on any tensor and are
+    tested without a device."""
+    import torch
+    if not isinstance(X, torch.Tensor):
+        raise TypeError("X must be a torch.Tensor, not %s" % type(X).__name__)
+    if X.dtype != torch.float64:
+        raise TypeError("X must be float64, not %s" % X.dtype)
+    if X.ndim != 2:
+        raise ValueError("X must be a 2-D [N, F] matrix, got shape %s" % (tuple(X.shape),))
+    columns = list(columns)
+    if len(columns) != X.shape[1]:
+        raise ValueError("%d columns named for %d in X" % (len(columns), X.shape[1]))
+    if len(set(columns)) != len(columns):
+        raise ValueError("columns must be distinct feature names")
+    if isinstance(y, torch.Tensor):
+        if y.is_cuda and y.device != X.device:
+            raise ValueError("y is on %s, X on %s" % (y.device, X.device))
+        if y.ndim != 1:
+            raise ValueError("y must be 1-D, got shape %s" % (tuple(y.shape),))
+        if y.dtype.is_complex:
+            raise TypeError("y must be bool, integer or floating, not %s" % y.dtype)
+        y = y.detach()
+        y = pd.Series((y.float() if y.dtype == torch.bfloat16 else y).cpu().numpy())     # float32 holds bfloat16 exactly
+    elif isinstance(y, pd.Series):
+        y = y.reset_index(drop=True)
+    elif isinstance(y, (np.ndarray, list)):
+        y = pd.Series(y)
+    else:
+        raise TypeError("y must be a torch.Tensor, numpy.ndarray, list or pandas.Series, not %s" % type(y).__name__)
+    return columns, y
+
+
+def _same_samples(X, y):
+    if len(X) != len(y):                 # a raise, not an assert: the library reads N targets
+        raise AssertionError("X and y must contain the same number of samples.")
+
+
+@contextlib.contextmanager
+def _bound_context(dev):
+    """The library context of `dev` with its calls enqueued on torch's current stream of the device, as
+    extract_features_device runs, so the matrix needs no synchronisation between extraction and selection."""
+    import torch
+    if dev.type != "cuda":
+        raise ValueError("X must be a CUDA tensor, got one on %s" % dev)
+    with torch.cuda.device(dev):
+        ctx = get_context(dev.index)
+        with ctx.lock:
+            ctx.set_stream(torch.cuda.current_stream(dev).cuda_stream or _lib.STREAM_LEGACY)
+            try:
+                yield ctx
+            finally:
+                ctx.set_stream(None)
+
+
+def _device_stats(X):
+    """(class_stats, regression_stats) of _relevance_table for the CUDA matrix X.  A row-major X (unit column stride,
+    row stride F) is read in place; any other layout, such as a column slice of a wider `out=`, is first copied by
+    torch into a contiguous scratch of N * F * 8 bytes."""
+    def run(select, *target):
+        with _bound_context(X.device) as ctx:
+            M = X.contiguous()
+            return select(ctx, M.data_ptr(), M.shape[0], M.shape[1], *target)
+    return (lambda codes, k: run(_lib.Context.select_classification_device, codes, k),
+            lambda yv: run(_lib.Context.select_regression_device, yv))
+
+
+def calculate_relevance_table_device(X, y, columns, *, ml_task="auto", multiclass=False, n_significant=1,
+                                     test_for_binary_target_real_feature=TEST_FOR_BINARY_TARGET_REAL_FEATURE,
+                                     fdr_level=FDR_LEVEL, hypotheses_independent=HYPOTHESES_INDEPENDENT, show_warnings=False):
+    """calculate_relevance_table of a feature matrix on the GPU, without a host copy of the matrix.
+
+    X: float64 CUDA tensor [N, F], rows are samples in positional order (e.g. the matrix extract_features_device
+    returns); columns: its F distinct feature names; y: N targets as a CUDA or CPU tensor (bool, integer or floating),
+    numpy array, list or pandas Series (taken positionally; string labels come through the host types).
+
+    Returns the table calculate_relevance_table(pd.DataFrame(X.cpu().numpy(), columns=columns), pd.Series(y)) returns,
+    with the same warnings and errors.  The statistics are computed on torch's current stream of X's device.  The host
+    waits for that stream to read them back: once for a classification target, and once per feature column for a
+    regression target (tsfx_select_regression reads each column's run count to choose its test).  A CUDA y adds one
+    copy to the host."""
+    columns, y = _device_args(X, y, columns)
+    _same_samples(X, y)
+    return _relevance_table(columns, y, *_device_stats(X), ml_task, multiclass, n_significant, show_warnings,
+                            test_for_binary_target_real_feature, fdr_level, hypotheses_independent)
+
+
+def select_features_device(X, y, columns, *, test_for_binary_target_binary_feature=TEST_FOR_BINARY_TARGET_BINARY_FEATURE,
+                           test_for_binary_target_real_feature=TEST_FOR_BINARY_TARGET_REAL_FEATURE,
+                           test_for_real_target_binary_feature=TEST_FOR_REAL_TARGET_BINARY_FEATURE,
+                           test_for_real_target_real_feature=TEST_FOR_REAL_TARGET_REAL_FEATURE, fdr_level=FDR_LEVEL,
+                           hypotheses_independent=HYPOTHESES_INDEPENDENT, n_jobs=N_PROCESSES, show_warnings=False,
+                           chunksize=None, ml_task="auto", multiclass=False, n_significant=1):
+    """select_features of a feature matrix on the GPU (arguments as calculate_relevance_table_device; the keywords are
+    select_features', whose `device` is X's device here).
+
+    Returns (X_sel, kept): X_sel a new float64 CUDA tensor [N, k] holding the relevant columns of X, kept their names,
+    in the order select_features gives them (the relevance table's).  With no relevant feature X_sel is [N, 0]."""
+    import torch
+    columns, y = _device_args(X, y, columns)
+    if not len(y) > 1:
+        raise AssertionError("y must contain at least two samples.")
+    _same_samples(X, y)
+    yh = y.to_numpy()
+    # len(set(y)) > 1 without boxing every number: NaN differs from everything, as boxed NaNs do in a set
+    if not ((yh != yh[0]).any() if yh.dtype.kind in "biuf" else len(set(yh)) > 1):
+        raise AssertionError("Feature selection is only possible if more than 1 label/class is provided")
+    table = _relevance_table(columns, y, *_device_stats(X), ml_task, multiclass, n_significant, show_warnings,
+                             test_for_binary_target_real_feature, fdr_level, hypotheses_independent)
+    kept = list(table[table.relevant].feature)
+    position = {c: i for i, c in enumerate(columns)}
+    index = torch.tensor([position[c] for c in kept], dtype=torch.int64, device=X.device)
+    return X.index_select(1, index), kept
