@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define TSFX_VERSION 2
+#define TSFX_VERSION 3
 
 /* error codes */
 #define TSFX_OK 0
@@ -241,9 +241,7 @@ int tsfx_extract_dense(tsfx_ctx* ctx, const tsfx_plan* plan, const float* values
  * previous blocks run and their result rows travel back.  Any other order is sorted on the device first.
  * Host pointers may be pageable (staged through pinned memory by worker threads) or page-locked.  With
  * TSFX_FLAG_DEVICE_PTRS every pointer (ids, sort_keys, values, out_ids, out) is a device pointer; the call still
- * synchronises once to learn the sizes.
- * Two-step use: call tsfx_build_csr with all output pointers NULL (it counts the series and keeps the CSR on the
- * device), size `out`, then call tsfx_extract_long with ids == values == NULL to extract from the held CSR. */
+ * synchronises once to learn the sizes. */
 int tsfx_extract_long(tsfx_ctx* ctx, const tsfx_plan* plan, const int64_t* ids, const void* sort_keys,
                       int32_t sort_key_is_f64, const float* values, int64_t n_rows, int64_t* out_ids,
                       double* out, int64_t out_capacity, int64_t* n_series_out, uint32_t flags);
@@ -287,12 +285,6 @@ void tsfx_host_free(tsfx_ctx* ctx, void* p);
 int tsfx_set_peer_outputs(tsfx_ctx* ctx, const uint64_t* peer_out, int32_t n_peers, int32_t self_index,
                           uint64_t multicast_out, int32_t mode);
 int tsfx_peer_flush(tsfx_ctx* ctx);
-
-/* Stage (a) alone: builds the CSR on the device (it stays held by the context until the next stage-(a)
- * call) and copies back whichever outputs are non-NULL. */
-int tsfx_build_csr(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
-                   const float* values, int64_t n_rows, int64_t* out_ids, int64_t* out_begin,
-                   int32_t* out_len, float* sorted_values, int64_t out_capacity, int64_t* n_series_out);
 
 /* roll_time_series as views: for every series s of the input CSR and every shift t of
  * dataframe_functions.py:340-373, 548-562 (positive rolling_direction: windows END at row t-1; negative: windows

@@ -97,6 +97,20 @@ def test_errors_like_the_reference():
     with pytest.raises(ValueError):
         extract_features([1, 2, 3], column_id="id")
 
+    # a NaN found on the device is the reference's error, naming the kind, with no library error chained to it
+    def nan_error(label, f, *args, **kw):
+        with pytest.raises(ValueError) as e:
+            f(*args, default_fc_parameters=MinimalFCParameters(), **kw)
+        assert str(e.value) == "Column must not contain NaN values: %s" % label and e.value.__suppress_context__
+    from tsfresh_b200 import do_extraction_on_chunks, roll_time_series
+    x = pd.Series(np.arange(20, dtype=np.float32))
+    nan_error("b", do_extraction_on_chunks, [(1, "a", x), (1, "b", x.where(x != 5))])
+    wide = df.assign(other=bad["value"])
+    nan_error("other", extract_features, roll_time_series(wide, column_id="id", column_sort="time", max_timeshift=3))
+    stacked = pd.concat([df.assign(kind="a"), bad.assign(kind="b")], ignore_index=True)
+    nan_error("b", extract_features, roll_time_series(stacked, column_id="id", column_sort="time", column_kind="kind",
+                                                      max_timeshift=3))
+
 
 def test_pivot_false_triples():
     series = list(synthetic_series(5, 3, 20))
@@ -259,7 +273,7 @@ def test_do_extraction_on_chunk_signature():
     assert len(out) == 2 * plan.n_cols + 2
 
 
-def test_wide_format_kind_dimension_on_the_device():
+def test_wide_format_kind_dimension_on_the_device(monkeypatch):
     """several value columns of one frame: ONE stage (a), per-kind settings, one result matrix (tsfx_extract_long_kinds);
     rows in order, shuffled, and with keys shuffled inside the ids -- same frame as the per-kind path"""
     rng = np.random.default_rng(31)
@@ -284,8 +298,11 @@ def test_wide_format_kind_dimension_on_the_device():
     for frame in (df.sample(frac=1.0, random_state=1), df.iloc[np.lexsort((rng.random(len(df)), ids))]):
         Y = extract_features(frame, column_id="id", column_sort="time", default_fc_parameters=s, kind_to_fc_parameters=per_kind)
         assert list(Y.columns) == list(X.columns) and np.array_equal(Y.to_numpy(), X.to_numpy(), equal_nan=True)
-    # a NaN in any kind is the reference's ValueError
+    # a NaN in any kind is the reference's ValueError: pandas' scan names the column, the device scan every value column
+    from tsfresh_b200 import extraction
     bad = df.copy()
     bad.loc[17, "b"] = np.nan
-    with pytest.raises(ValueError, match="NaN"):
-        extract_features(bad, column_id="id", column_sort="time", default_fc_parameters=MinimalFCParameters())
+    for limit, label in ((1 << 20, "b"), (0, "a, b, 7")):
+        monkeypatch.setattr(extraction, "_HOST_NAN_CHECK_ROWS", limit)
+        with pytest.raises(ValueError, match="^Column must not contain NaN values: %s$" % label):
+            extract_features(bad, column_id="id", column_sort="time", default_fc_parameters=MinimalFCParameters())

@@ -240,7 +240,7 @@ def test_errors_before_any_kernel_group():
 
     bad = x.clone()
     bad[57, 100] = float("nan")
-    raises(ValueError, "NaN", bad, default_fc_parameters=s)
+    raises(ValueError, "^Column must not contain NaN values: 0$", bad, default_fc_parameters=s)
     vals = x.reshape(-1)
     R = vals.numel()
     begin = torch.arange(50, device=DEV, dtype=torch.int64) * 300
@@ -251,7 +251,7 @@ def test_errors_before_any_kernel_group():
         raises(ValueError, r"series %d has an invalid \(begin, len\)" % series, vals, b, ln, default_fc_parameters=s)
     nanv = vals.clone()
     nanv[int(begin[8]) + 255] = float("nan")
-    raises(ValueError, "NaN", nanv, begin, length, default_fc_parameters=s)
+    raises(ValueError, "^Column must not contain NaN values: 0$", nanv, begin, length, default_fc_parameters=s)
     long = torch.zeros(131_073 + 200, device=DEV)
     raises(ValueError, "exceeds", long, torch.tensor([0, 100, 131_173], device=DEV),
            torch.tensor([100, 131_073, 100], device=DEV), default_fc_parameters=s)

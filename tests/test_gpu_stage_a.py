@@ -1,4 +1,4 @@
-"""Stage (a) of the hot path through the C ABI (tsfx_extract_long_alloc / tsfx_extract_long / tsfx_build_csr):
+"""Stage (a) of the hot path through the C ABI (tsfx_extract_long_alloc / tsfx_extract_long / tsfx_extract_long_kinds):
 the pipelined path for rows ordered by (id, sort key), the device sort for every other order, the NaN scan, pinned
 and pageable host buffers, device pointers.  Restates the reference's adapter behaviour
 (tsfresh/feature_extraction/data.py:217-230, 280-291; row-order invariance: test_extraction.py:207-237)."""
@@ -96,6 +96,15 @@ def test_nan_values_are_an_error(env):
     v[len(v) // 2] = 0.0
     uid2, mat = dp.extract_long(ids, t, v)
     assert np.isfinite(mat).all()
+    # no ids / values but rows to read is a bad call, whatever the previous call left on the device
+    import ctypes
+    n = ctypes.c_int64(0)
+    out_ids, out = np.empty(len(uid2), np.int64), np.empty((len(uid2), plan.n_cols))
+    rc = ctx.lib.tsfx_extract_long(ctx.h, dp.h, None, None, 0, None, len(ids), ctypes.c_void_p(out_ids.ctypes.data),
+                                   ctypes.c_void_p(out.ctypes.data), len(uid2), ctypes.byref(n), 0)
+    assert rc == -1 and n.value == 0
+    with pytest.raises(ValueError, match="tsfx_extract_long: bad arguments"):
+        ctx.check(rc, "tsfx_extract_long")
 
 
 def test_extract_features_reports_the_nan_column():

@@ -34,7 +34,7 @@ class FakeLib:
     def _record(self, name, X, n, f, flags):
         matrix = self._array(X, n * f).reshape(n, f).copy() if f else None
         self.calls.append({"name": name, "ptr": X.value, "flags": flags, "matrix": matrix})
-        return -4 if self.nan else 0
+        return -6 if self.nan else 0                 # TSFX_E_NAN
 
     def tsfx_select_classification(self, h, X, n, f, y, k, out, flags):
         rc = self._record("classification", X, n, f, flags)
@@ -157,6 +157,13 @@ def test_nan_in_the_matrix(monkeypatch):
     for y in (Y2, np.linspace(0, 1, N)):
         with pytest.raises(ValueError, match="Feature matrix contains NaN values"):
             calculate_relevance_table_device(matrix(), y, COLUMNS)
+
+
+def test_nan_status_is_a_typed_value_error():
+    ctx = fake_context(FakeLib(nan=True))
+    with pytest.raises(_lib.NanValuesError, match="^tsfx_select_regression: the feature matrix contains NaN$") as e:
+        ctx.select_regression(np.zeros((N, 3)), np.zeros(N))
+    assert isinstance(e.value, ValueError)
 
 
 def tables(X, y, columns, **kw):

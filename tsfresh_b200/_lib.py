@@ -22,14 +22,19 @@ STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy d
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
 
-_ERR = {-1: ValueError, -2: RuntimeError, -3: NotImplementedError, -4: ValueError, -5: MemoryError, -6: ValueError}
+
+class NanValuesError(ValueError):
+    """TSFX_E_NAN: the input holds a NaN value (the reference refuses such columns)."""
+
+
+_ERR = {-1: ValueError, -2: RuntimeError, -3: NotImplementedError, -4: ValueError, -5: MemoryError, -6: NanValuesError}
 
 _lib = None
 _lock = threading.Lock()
 
 EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync", "tsfx_version",
            "tsfx_plan_create", "tsfx_plan_destroy", "tsfx_extract_csr", "tsfx_extract_dense",
-           "tsfx_extract_long", "tsfx_build_csr", "tsfx_roll_windows", "tsfx_get_timings",
+           "tsfx_extract_long", "tsfx_roll_windows", "tsfx_get_timings",
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
            "tsfx_ctx_set_stream", "tsfx_set_out_ld"]
@@ -58,7 +63,6 @@ def load():
         lib.tsfx_extract_csr.argtypes = [vp, vp, vp, i64, vp, vp, i64, vp, u32]
         lib.tsfx_extract_dense.argtypes = [vp, vp, vp, i64, i32, vp, u32]
         lib.tsfx_extract_long.argtypes = [vp, vp, vp, vp, i32, vp, i64, vp, vp, i64, ctypes.POINTER(i64), u32]
-        lib.tsfx_build_csr.argtypes = [vp, vp, vp, i32, vp, i64, vp, vp, vp, vp, i64, ctypes.POINTER(i64)]
         lib.tsfx_roll_windows.argtypes = [vp, vp, i64, i32, i32, i32, vp, vp, vp, vp, i64]
         lib.tsfx_roll_windows.restype = i64
         lib.tsfx_get_timings.argtypes = [vp, vp, vp, i32]
@@ -101,6 +105,16 @@ def kernel_variants():
 
 def _ptr(a):
     return None if a is None else ctypes.c_void_p(a.ctypes.data)
+
+
+def _sort_key_array(sort_keys):
+    """(contiguous int64 or float64 sort keys or None, is_f64 flag of the C ABI)"""
+    if sort_keys is None:
+        return None, 0
+    sort_keys = np.asarray(sort_keys)
+    if sort_keys.dtype.kind == "f":
+        return np.ascontiguousarray(sort_keys, dtype=np.float64), 1
+    return np.ascontiguousarray(sort_keys, dtype=np.int64), 0
 
 
 class Context:
@@ -320,14 +334,7 @@ class DevicePlan:
         times: int64 ns timestamp of every row (the frame's DatetimeIndex) when the plan has linear_trend_timewise."""
         ids = np.ascontiguousarray(ids, dtype=np.int64)
         values = np.ascontiguousarray(values, dtype=np.float32)
-        is_f64 = 0
-        if sort_keys is not None:
-            sort_keys = np.asarray(sort_keys)
-            if sort_keys.dtype.kind == "f":
-                sort_keys = np.ascontiguousarray(sort_keys, dtype=np.float64)
-                is_f64 = 1
-            else:
-                sort_keys = np.ascontiguousarray(sort_keys, dtype=np.int64)
+        sort_keys, is_f64 = _sort_key_array(sort_keys)
         n_series = ctypes.c_int64(0)
         p_ids, p_out = ctypes.c_void_p(), ctypes.c_void_p()
         ctx = self.ctx
@@ -337,16 +344,11 @@ class DevicePlan:
             rc = ctx.lib.tsfx_extract_long_alloc(ctx.h, self.h, _ptr(ids), _ptr(sort_keys), is_f64, _ptr(values), len(ids),
                                                  ctypes.byref(p_ids), ctypes.byref(p_out), ctypes.byref(n_series), flags)
             ctx.check(rc, "tsfx_extract_long")
-        k = n_series.value
-        if k == 0 or not p_out.value:
-            return np.empty(0, dtype=np.int64), np.empty((0, self.n_cols), dtype=np.float64)
-        return ctx._wrap_pinned(p_ids.value, (k,), np.int64), ctx._wrap_pinned(p_out.value, (k, self.n_cols), np.float64)
+        return _pooled_result(ctx, p_ids, p_out, n_series.value, self.n_cols)
 
     def extract_long_into(self, ids, sort_keys, values, out_ids, out, flags=0):
         """tsfx_extract_long into caller buffers (rows of a larger pinned matrix): returns the number of series written"""
-        is_f64 = 0
-        if sort_keys is not None and sort_keys.dtype.kind == "f":
-            is_f64 = 1
+        sort_keys, is_f64 = _sort_key_array(sort_keys)
         n_series = ctypes.c_int64(0)
         ctx = self.ctx
         with ctx.lock:
@@ -356,32 +358,20 @@ class DevicePlan:
         return n_series.value
 
     # ---- device-pointer entry points (torch tensors own the memory) ----------------------------
-    def extract_dense_device(self, values_ptr, n_series, length, out_ptr, timing=False):
-        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0)
+    # checked: the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT) first validates the views, measures the longest one and
+    # scans the values for NaN on the device, before any kernel group runs
+    def extract_dense_device(self, values_ptr, n_series, length, out_ptr, timing=False, checked=False):
+        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0)
         rc = self.ctx.lib.tsfx_extract_dense(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_series, length,
                                              ctypes.c_void_p(out_ptr), flags)
         self.ctx.check(rc, "tsfx_extract_dense")
 
-    def extract_dense_checked(self, values_ptr, n_series, length, out_ptr):
-        """tsfx_extract_dense on device pointers after the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT)"""
-        flags = FLAG_DEVICE_PTRS | FLAG_CHECK_DEVICE_INPUT
-        rc = self.ctx.lib.tsfx_extract_dense(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_series, length,
-                                             ctypes.c_void_p(out_ptr), flags)
-        self.ctx.check(rc, "tsfx_extract_dense")
-
-    def extract_csr_checked(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr):
-        """tsfx_extract_csr on device pointers after the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT): the views are
-        validated and the longest one measured on the device, whatever tsfx_set_max_len_hint holds"""
-        flags = FLAG_DEVICE_PTRS | FLAG_CHECK_DEVICE_INPUT
-        rc = self.ctx.lib.tsfx_extract_csr(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_values,
-                                           ctypes.c_void_p(begin_ptr), ctypes.c_void_p(len_ptr), n_series,
-                                           ctypes.c_void_p(out_ptr), flags)
-        self.ctx.check(rc, "tsfx_extract_csr")
-
-    def extract_csr_device(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr, timing=False, max_len=0):
-        """max_len: upper bound of the series lengths if the caller knows one (keeps the call asynchronous)"""
-        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0)
-        self.ctx.check(self.ctx.lib.tsfx_set_max_len_hint(self.ctx.h, int(max_len)), "tsfx_set_max_len_hint")
+    def extract_csr_device(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr, timing=False, max_len=0,
+                           checked=False):
+        """max_len: upper bound of the series lengths if the caller knows one (keeps an unchecked call asynchronous)"""
+        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0)
+        if not checked:
+            self.ctx.check(self.ctx.lib.tsfx_set_max_len_hint(self.ctx.h, int(max_len)), "tsfx_set_max_len_hint")
         rc = self.ctx.lib.tsfx_extract_csr(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_values,
                                            ctypes.c_void_p(begin_ptr), ctypes.c_void_p(len_ptr), n_series,
                                            ctypes.c_void_p(out_ptr), flags)
@@ -394,14 +384,7 @@ def extract_long_kinds(ctx, device_plans, ids, sort_keys, value_columns, flags=0
     ids = np.ascontiguousarray(ids, dtype=np.int64)
     cols = [np.ascontiguousarray(v, dtype=np.float32) for v in value_columns]
     assert len(cols) == len(device_plans) and all(len(c) == len(ids) for c in cols)
-    is_f64 = 0
-    if sort_keys is not None:
-        sort_keys = np.asarray(sort_keys)
-        if sort_keys.dtype.kind == "f":
-            sort_keys = np.ascontiguousarray(sort_keys, dtype=np.float64)
-            is_f64 = 1
-        else:
-            sort_keys = np.ascontiguousarray(sort_keys, dtype=np.int64)
+    sort_keys, is_f64 = _sort_key_array(sort_keys)
     K = len(cols)
     plan_arr = (ctypes.c_void_p * K)(*[dp.h for dp in device_plans])
     val_arr = (ctypes.c_void_p * K)(*[c.ctypes.data for c in cols])
@@ -414,36 +397,14 @@ def extract_long_kinds(ctx, device_plans, ids, sort_keys, value_columns, flags=0
         rc = ctx.lib.tsfx_extract_long_kinds(ctx.h, plan_arr, _ptr(ids), _ptr(sort_keys), is_f64, val_arr, K, len(ids),
                                              ctypes.byref(p_ids), ctypes.byref(p_out), ctypes.byref(n_series), flags)
         ctx.check(rc, "tsfx_extract_long_kinds")
-    k = n_series.value
+    return _pooled_result(ctx, p_ids, p_out, n_series.value, total)
+
+
+def _pooled_result(ctx, p_ids, p_out, k, n_cols):
+    """(unique ids, [k x n_cols] matrix) that a tsfx_extract_long_alloc / _kinds call returned on the pinned pool"""
     if k == 0 or not p_out.value:
-        return np.empty(0, dtype=np.int64), np.empty((0, total), dtype=np.float64)
-    return ctx._wrap_pinned(p_ids.value, (k,), np.int64), ctx._wrap_pinned(p_out.value, (k, total), np.float64)
-
-
-def build_csr(ctx, ids, sort_keys, values):
-    """Stage (a) alone: returns (unique_ids, begin, len, values_in_series_order)."""
-    ids = np.ascontiguousarray(ids, dtype=np.int64)
-    values = np.ascontiguousarray(values, dtype=np.float32)
-    is_f64 = 0
-    if sort_keys is not None:
-        sort_keys = np.asarray(sort_keys)
-        if sort_keys.dtype.kind == "f":
-            sort_keys = np.ascontiguousarray(sort_keys, dtype=np.float64)
-            is_f64 = 1
-        else:
-            sort_keys = np.ascontiguousarray(sort_keys, dtype=np.int64)
-    n = len(ids)
-    uid = np.empty(n, dtype=np.int64)
-    begin = np.empty(n, dtype=np.int64)
-    length = np.empty(n, dtype=np.int32)
-    sv = np.empty(n, dtype=np.float32)
-    k = ctypes.c_int64(0)
-    with ctx.lock:
-        rc = ctx.lib.tsfx_build_csr(ctx.h, _ptr(ids), _ptr(sort_keys), is_f64, _ptr(values), n, _ptr(uid), _ptr(begin),
-                                    _ptr(length), _ptr(sv), n, ctypes.byref(k))
-        ctx.check(rc, "tsfx_build_csr")
-    k = k.value
-    return uid[:k].copy(), begin[:k].copy(), length[:k].copy(), sv
+        return np.empty(0, dtype=np.int64), np.empty((0, n_cols), dtype=np.float64)
+    return ctx._wrap_pinned(p_ids.value, (k,), np.int64), ctx._wrap_pinned(p_out.value, (k, n_cols), np.float64)
 
 
 def roll_windows(begin, length, rolling_direction, max_timeshift, min_timeshift):

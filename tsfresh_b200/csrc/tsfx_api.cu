@@ -252,8 +252,6 @@ struct tsfx_ctx {
     ImputeWorkspace imp;
     SelectWorkspace sel;
     DevBuf sel_x, sel_y, sel_out;
-    int64_t held_series = -1;    // CSR kept on the device by the last stage-(a) call (-1: none)
-    int held_max_len = 0;
     bool used_moments = false;   // the last pass ran k_moments in place of k_basic (reported as "moments")
     DevBuf kvals, kvals_sorted;  // value columns of kinds 1 .. K-1 of a wide frame (input order / CSR order)
     DevBuf times, times_sorted;  // tsfx_set_row_times: row timestamps of the next extract call (linear_trend_timewise)
@@ -1223,56 +1221,6 @@ static int stage_a_sort(tsfx_ctx* ctx, const LongIn& in, int max_blocks, bool ch
     return TSFX_OK;
 }
 
-extern "C" int tsfx_build_csr(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
-                              const float* values, int64_t n_rows, int64_t* out_ids, int64_t* out_begin,
-                              int32_t* out_len, float* sorted_values, int64_t out_capacity, int64_t* n_series_out) {
-    if (!ctx) return TSFX_E_INVALID;
-    if (n_rows < 0 || !n_series_out || (n_rows > 0 && (!ids || !values)))
-        return fail(ctx, TSFX_E_INVALID, "tsfx_build_csr: bad arguments");
-    CK(cudaSetDevice(ctx->device));
-    *n_series_out = 0;
-    if (n_rows == 0) return TSFX_OK;
-    ctx->held_series = -1;
-    LongIn in{ids, sort_keys, sort_key_is_f64, values, n_rows, false};
-    CsrInfo info;
-    bool streamed = false;
-    const int64_t* d_ids; const uint64_t* d_keys; const float* d_vals;
-    int rc = stage_a(ctx, in, 1, true, &info, &streamed, &d_ids, &d_keys, &d_vals);
-    if (rc) return rc;
-    CsrWorkspace& W = ctx->csr;
-    bool need_sort = info.unsorted_ids != 0;
-    if (!need_sort) {        // ids ascending: bring the other columns over and look inside the ids
-        if (sort_keys) CK(ctx->stager.h2d(W.keys(), sort_keys, (size_t)n_rows * 8, ctx->stream));
-        CK(ctx->stager.h2d(W.vals(), values, (size_t)n_rows * 4, ctx->stream));
-        csr_check_rows(W, d_ids, d_keys, sort_key_is_f64, d_vals, 0, n_rows, true, ctx->stream);
-        CK(cudaMemcpyAsync(W.h_info, W.d_info, sizeof(CsrInfo), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        info = *W.h_info;
-        need_sort = info.unsorted_keys != 0;
-        if (need_sort) {     // columns are resident now: sort in place
-            LongIn dev{d_ids, d_keys, sort_key_is_f64, d_vals, n_rows, true};
-            rc = stage_a_sort(ctx, dev, 1, true, &info, d_ids, d_keys, d_vals);
-            if (rc) return rc;
-        }
-    } else {
-        rc = stage_a_sort(ctx, in, 1, true, &info, d_ids, d_keys, d_vals);
-        if (rc) return rc;
-    }
-    if (info.has_nan) return nan_error(ctx);
-    const int64_t ns = info.n_series;
-    ctx->held_series = ns;
-    ctx->held_max_len = info.max_len;
-    *n_series_out = ns;
-    if (!out_ids && !out_begin && !out_len && !sorted_values) return TSFX_OK;      // count + keep on device
-    if (ns > out_capacity) return fail(ctx, TSFX_E_INVALID, "out_capacity too small: " + std::to_string(ns) + " series");
-    if (out_ids) CK(cudaMemcpyAsync(out_ids, W.d_uid, ns * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_begin) CK(cudaMemcpyAsync(out_begin, W.d_begin, ns * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (out_len) CK(cudaMemcpyAsync(out_len, W.d_len, ns * sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
-    if (sorted_values) CK(cudaMemcpyAsync(sorted_values, W.d_values, n_rows * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    return TSFX_OK;
-}
-
 // the kinds of one call: plan, device value column (CSR order) and first output column of each
 #define TSFX_MAX_KINDS 64
 struct KindSet {
@@ -1355,7 +1303,6 @@ static int extract_long_impl(tsfx_ctx* ctx, const tsfx_plan* const* plans, const
     if (K.n > 1 && !in.device) CK(ctx->kvals.reserve((size_t)(K.n - 1) * kstride * 4 + 16));
     const bool check_nan = !(flags & TSFX_FLAG_NO_NAN_CHECK);
     const int max_blocks = (flags & TSFX_FLAG_TIMING) ? 1 : 16;
-    ctx->held_series = -1;
     const int64_t* times_in = nullptr;           // row timestamps (input row order), device
     int rc = take_times(ctx, plan, in.n, &times_in);
     if (rc) return rc;
@@ -1442,8 +1389,6 @@ static int extract_long_impl(tsfx_ctx* ctx, const tsfx_plan* const* plans, const
             streamed = false;
         }
     }
-    ctx->held_series = info.n_series;
-    ctx->held_max_len = info.max_len;
     return TSFX_OK;
 }
 
@@ -1452,34 +1397,31 @@ extern "C" int tsfx_extract_long(tsfx_ctx* ctx, const tsfx_plan* plan, const int
                                  double* out, int64_t out_capacity, int64_t* n_series_out, uint32_t flags) {
     if (!ctx) return TSFX_E_INVALID;
     if (!plan || plan->ctx != ctx) return fail(ctx, TSFX_E_INVALID, "plan does not belong to this context");
-    const bool reuse = (ids == nullptr && values == nullptr);     // run on the CSR held from tsfx_build_csr
-    if (n_rows < 0 || !n_series_out || (!reuse && n_rows > 0 && (!ids || !values)) || !out)
+    if (n_rows < 0 || !n_series_out || (n_rows > 0 && (!ids || !values)) || !out)
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long: bad arguments");
     CK(cudaSetDevice(ctx->device));
     *n_series_out = 0;
-    if (reuse) {
-        if (flags & TSFX_FLAG_DEVICE_PTRS) return fail(ctx, TSFX_E_INVALID, "the held CSR is extracted into host buffers");
-        if (ctx->held_series < 0) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long: no CSR is held by this context");
-        if (plan->need_times) return fail(ctx, TSFX_E_UNSUPPORTED, "linear_trend_timewise: use the one-call form of tsfx_extract_long");
-        const int64_t ns = ctx->held_series;
-        *n_series_out = ns;
-        if (ns == 0) return TSFX_OK;
-        if (ns > out_capacity) return fail(ctx, TSFX_E_INVALID, "out_capacity too small: " + std::to_string(ns) + " series");
-        CsrInfo info = {};
-        info.n_series = ns; info.max_len = ctx->held_max_len; info.n_blocks = 1;
-        info.series_lo[0] = 0; info.series_lo[1] = ns; info.row_lo[0] = 0; info.row_lo[1] = 0;
-        KindSet K1;
-        K1.plan[0] = plan; K1.dvals[0] = ctx->csr.d_values; K1.col0[0] = 0; K1.total_cols = plan->ncols;
-        int rc = run_blocks(ctx, K1, info, nullptr, nullptr, nullptr, false, false, out, false, flags);
-        if (rc) return rc;
-        if (out_ids) CK(cudaMemcpyAsync(out_ids, ctx->csr.d_uid, ns * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->s_out));
-        CK(cudaStreamSynchronize(ctx->stream));
-        return TSFX_OK;
-    }
     if (n_rows == 0) return TSFX_OK;
     LongIn in{ids, sort_keys, sort_key_is_f64, values, n_rows, (flags & TSFX_FLAG_DEVICE_PTRS) != 0};
     return extract_long_impl(ctx, &plan, in, out_ids, out, out_capacity, nullptr, nullptr, n_series_out, flags);
+}
+
+// tsfx_extract_long_alloc / _kinds after their argument checks: the result comes from the pinned pool, and goes back to
+// it when the call fails
+static int extract_long_pooled(tsfx_ctx* ctx, const tsfx_plan* const* plans, const LongIn& in, int64_t** out_ids,
+                               double** out, int64_t* n_series_out, uint32_t flags) {
+    CK(cudaSetDevice(ctx->device));
+    *n_series_out = 0;
+    *out = nullptr;
+    *out_ids = nullptr;
+    if (in.n == 0) return TSFX_OK;
+    int rc = extract_long_impl(ctx, plans, in, nullptr, nullptr, 0, out_ids, out, n_series_out, flags);
+    if (rc) {
+        if (*out) ctx->pool.free(*out);
+        if (*out_ids) ctx->pool.free(*out_ids);
+        *out = nullptr; *out_ids = nullptr;
+    }
+    return rc;
 }
 
 extern "C" int tsfx_extract_long_alloc(tsfx_ctx* ctx, const tsfx_plan* plan, const int64_t* ids, const void* sort_keys,
@@ -1490,19 +1432,8 @@ extern "C" int tsfx_extract_long_alloc(tsfx_ctx* ctx, const tsfx_plan* plan, con
     if (flags & TSFX_FLAG_DEVICE_PTRS) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_alloc takes host pointers");
     if (n_rows < 0 || !n_series_out || !out || !out_ids || (n_rows > 0 && (!ids || !values)))
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_alloc: bad arguments");
-    CK(cudaSetDevice(ctx->device));
-    *n_series_out = 0;
-    *out = nullptr;
-    *out_ids = nullptr;
-    if (n_rows == 0) return TSFX_OK;
-    LongIn in{ids, sort_keys, sort_key_is_f64, values, n_rows, false};
-    int rc = extract_long_impl(ctx, &plan, in, nullptr, nullptr, 0, out_ids, out, n_series_out, flags);
-    if (rc) {
-        if (*out) ctx->pool.free(*out);
-        if (*out_ids) ctx->pool.free(*out_ids);
-        *out = nullptr; *out_ids = nullptr;
-    }
-    return rc;
+    return extract_long_pooled(ctx, &plan, LongIn{ids, sort_keys, sort_key_is_f64, values, n_rows, false}, out_ids, out,
+                               n_series_out, flags);
 }
 
 extern "C" int tsfx_extract_long_kinds(tsfx_ctx* ctx, const tsfx_plan* const* plans, const int64_t* ids, const void* sort_keys,
@@ -1515,21 +1446,10 @@ extern "C" int tsfx_extract_long_kinds(tsfx_ctx* ctx, const tsfx_plan* const* pl
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_kinds: bad arguments");
     for (int k = 0; k < n_kinds; ++k)
         if (!plans[k] || (n_rows > 0 && !values[k])) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_kinds: NULL plan / column");
-    CK(cudaSetDevice(ctx->device));
-    *n_series_out = 0;
-    *out = nullptr;
-    *out_ids = nullptr;
-    if (n_rows == 0) return TSFX_OK;
     LongIn in{ids, sort_keys, sort_key_is_f64, values[0], n_rows, false};
     in.more = values + 1;
     in.n_kinds = n_kinds;
-    int rc = extract_long_impl(ctx, plans, in, nullptr, nullptr, 0, out_ids, out, n_series_out, flags);
-    if (rc) {
-        if (*out) ctx->pool.free(*out);
-        if (*out_ids) ctx->pool.free(*out_ids);
-        *out = nullptr; *out_ids = nullptr;
-    }
-    return rc;
+    return extract_long_pooled(ctx, plans, in, out_ids, out, n_series_out, flags);
 }
 
 extern "C" void* tsfx_host_alloc(tsfx_ctx* ctx, size_t bytes) {

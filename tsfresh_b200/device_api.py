@@ -14,9 +14,7 @@ import pandas as pd
 
 from . import _lib
 from .dataframe_functions import impute, impute_dataframe_zero
-from .extraction import _check_colname, _device_plan, get_context
-from .plan import Plan
-from .settings import ComprehensiveFCParameters
+from .extraction import _check_colname, _default_settings, _device_plan, _kind_plan, _nan_column, get_context
 
 
 def _layout(values, begin, length, kinds):
@@ -63,16 +61,12 @@ def _layout(values, begin, length, kinds):
 
 def _plans(kinds, default_fc_parameters, kind_to_fc_parameters):
     """One Plan per kind and the result's column names, as extract_features gives them for a wide frame."""
-    if default_fc_parameters is None and kind_to_fc_parameters is None:
-        default_fc_parameters = ComprehensiveFCParameters()
-    elif default_fc_parameters is None:
-        default_fc_parameters = {}
+    default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
     plans, columns = [], []
     for kind in kinds:
-        fc = kind_to_fc_parameters[kind] if (kind_to_fc_parameters and kind in kind_to_fc_parameters) else default_fc_parameters
-        plan = Plan(fc, has_datetime_index=False)
+        plan, names = _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters)
         plans.append(plan)
-        columns += [str(kind) + "__" + s for s in plan.suffixes]
+        columns += names
     return plans, columns
 
 
@@ -143,15 +137,11 @@ def extract_features_device(values, begin=None, length=None, *, default_fc_param
                         col = v.contiguous()
                     dp = _device_plan(ctx, plan)
                     o = target.data_ptr() + c0 * 8
-                    try:
+                    with _nan_column(kinds[k]):
                         if csr:
-                            dp.extract_csr_checked(col.data_ptr(), col.shape[0], b.data_ptr(), ln.data_ptr(), n, o)
+                            dp.extract_csr_device(col.data_ptr(), col.shape[0], b.data_ptr(), ln.data_ptr(), n, o, checked=True)
                         else:
-                            dp.extract_dense_checked(col.data_ptr(), n, col.shape[1], o)
-                    except ValueError as e:
-                        if "contains NaN" in str(e):        # data.py:148-167, the check every extraction path makes
-                            raise ValueError("Column must not contain NaN values: {}".format(kinds[k])) from None
-                        raise
+                            dp.extract_dense_device(col.data_ptr(), n, col.shape[1], o, checked=True)
                     c0 += plan.n_cols
                 if mode is not None:
                     ctx.impute_device(target.data_ptr(), n, width, mode)

@@ -11,8 +11,6 @@ pivots the returned (id, name, value) triples (data.py:86-121).  The Python `map
 """
 import numpy as np
 
-from .plan import Plan
-
 
 def _reference_base():
     try:
@@ -73,12 +71,9 @@ class CsrTsData(_reference_tsdata_base()):
             raise ValueError("begin, length and ids must have one entry per series")
 
     def apply(self, f, meta=None, default_fc_parameters=None, kind_to_fc_parameters=None, **_):
-        from .extraction import _device_plan, get_context
-        fc = (kind_to_fc_parameters or {}).get(self.kind, default_fc_parameters or {})
-        plan = Plan(fc)
-        dp = _device_plan(get_context(self.device), plan)
-        mat = dp.extract_csr(self.values, self.begin, self.length)
-        return [self.kind + "__" + s for s in plan.suffixes], mat
+        from .extraction import _device_plan, _kind_plan, get_context
+        plan, names = _kind_plan(self.kind, default_fc_parameters or {}, kind_to_fc_parameters)
+        return names, _device_plan(get_context(self.device), plan).extract_csr(self.values, self.begin, self.length)
 
     def pivot(self, results):
         import pandas as pd

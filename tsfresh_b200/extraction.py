@@ -16,6 +16,7 @@ Differences that are part of the contract (BASELINE.json north_star):
     pinned result matrix; `device=` or a torchrun LOCAL_RANK pins the call to one GPU (one process per GPU, see
     tsfresh_b200.distributed).  chunksize / profile* are accepted for signature compatibility.
 """
+import contextlib
 import threading
 import warnings
 
@@ -53,6 +54,48 @@ def _device_plan(ctx, plan):
         dp = _lib.DevicePlan(ctx, plan)
         ctx._plans[key] = dp
     return dp
+
+
+def _default_settings(default_fc_parameters, kind_to_fc_parameters):
+    """extraction.py:149-152: no settings at all is ComprehensiveFCParameters; per-kind settings alone leave the other
+    kinds without features."""
+    if default_fc_parameters is None:
+        return ComprehensiveFCParameters() if kind_to_fc_parameters is None else {}
+    return default_fc_parameters
+
+
+def _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters, has_datetime_index=False, show_warnings=False):
+    """(Plan, column names) of one kind.  The settings are looked up with the RAW kind (extraction.py:333-336), the
+    names carry str(kind) (:374-378)."""
+    if kind_to_fc_parameters and kind in kind_to_fc_parameters:
+        fc = kind_to_fc_parameters[kind]
+    else:
+        fc = default_fc_parameters
+    plan = Plan(fc, has_datetime_index=has_datetime_index)
+    if show_warnings:
+        for name in plan.skipped:
+            warnings.warn("{} requires the data to have a index of type {}. Results will "
+                          "not be calculated".format(name, pd.DatetimeIndex))
+    return plan, [str(kind) + "__" + sfx for sfx in plan.suffixes]
+
+
+@contextlib.contextmanager
+def _nan_column(label):
+    """Turns TSFX_E_NAN (a NaN found by the device's scan of the values) into the reference's error for the column(s)
+    `label` (data.py:148-167)."""
+    try:
+        yield
+    except _lib.NanValuesError:
+        raise ValueError("Column must not contain NaN values: {}".format(label)) from None
+
+
+def _impute_on_device(ctx, result):
+    """impute(result) (dataframe_functions.py:49-77) by one tsfx_impute pass, as a new frame"""
+    if not (result.shape[0] and result.shape[1]):
+        return result
+    m = np.ascontiguousarray(result.to_numpy(dtype=np.float64))
+    ctx.impute(m, _lib.IMPUTE_RANGE)
+    return pd.DataFrame(m, index=result.index, columns=result.columns, copy=False)
 
 
 # ------------------------------------------------------------------ validation (data.py:124-167)
@@ -246,16 +289,7 @@ def do_extraction_on_chunks(chunks, default_fc_parameters, kind_to_fc_parameters
         order.append(None)
     results = [None] * len(order)
     for (kind, is_dt), items in by_kind.items():
-        if kind_to_fc_parameters and kind in kind_to_fc_parameters:
-            fc = kind_to_fc_parameters[kind]
-        else:
-            fc = default_fc_parameters
-        plan = Plan(fc, has_datetime_index=is_dt)
-        if show_warnings:
-            for name in plan.skipped:
-                warnings.warn("{} requires the data to have a index of type {}. Results will "
-                              "not be calculated".format(name, pd.DatetimeIndex))
-        names = [str(kind) + "__" + sfx for sfx in plan.suffixes]
+        plan, names = _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters, is_dt, show_warnings)
         if plan.n_cols == 0:
             for pos, sid, _ in items:
                 results[pos] = []
@@ -268,12 +302,8 @@ def do_extraction_on_chunks(chunks, default_fc_parameters, kind_to_fc_parameters
         times = None
         if plan.needs_times:
             times = np.concatenate([d.index.as_unit("ns").asi8 for _, _, d in items])
-        try:
+        with _nan_column(kind):
             mat = _device_plan(ctx, plan).extract_csr(np.concatenate(vals), begin, lens, times=times)
-        except ValueError as e:
-            if "contains NaN" in str(e):
-                raise ValueError("Column must not contain NaN values: {}".format(kind)) from None
-            raise
         for r, (pos, sid, _) in enumerate(items):
             results[pos] = [(sid, n, mat[r, c]) for c, n in enumerate(names)]
     return [t for chunk in results for t in chunk]
@@ -295,17 +325,11 @@ def _extract_rolled(rolled, default_fc_parameters, kind_to_fc_parameters, impute
     device_impute = impute_function is _dff.impute
 
     def run(kind, values, begin, length, flags):
-        fc = kind_to_fc_parameters[kind] if (kind_to_fc_parameters and kind in kind_to_fc_parameters) else default_fc_parameters
-        plan = Plan(fc)
-        names = [kind + "__" + s for s in plan.suffixes]
+        plan, names = _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters)
         if plan.n_cols == 0 or len(begin) == 0:
             return names, np.empty((len(begin), plan.n_cols))
-        try:
+        with _nan_column(kind):           # the reference raises this while adapting the rolled frame
             return names, _device_plan(ctx, plan).extract_csr(values, begin, length, flags=flags)
-        except ValueError as e:
-            if "contains NaN" in str(e):      # the reference raises this while adapting the rolled frame (data.py:148-167)
-                raise ValueError("Column must not contain NaN values: {}".format(kind)) from None
-            raise
 
     if rolled.parts is None:                 # wide frame: every kind shares the windows
         flags = _lib.FLAG_IMPUTE if device_impute else 0          # columns are independent: per-kind impute is exact
@@ -337,10 +361,7 @@ def _extract_rolled(rolled, default_fc_parameters, kind_to_fc_parameters, impute
     result = pd.DataFrame(data, index=index, columns=columns, copy=False)
     if impute_function is not None and not imputed:
         if device_impute:
-            if result.shape[0] and result.shape[1]:
-                m = np.ascontiguousarray(result.to_numpy(dtype=np.float64))
-                ctx.impute(m, _lib.IMPUTE_RANGE)
-                result = pd.DataFrame(m, index=result.index, columns=result.columns, copy=False)
+            result = _impute_on_device(ctx, result)
         else:
             impute_function(result)
     return result
@@ -354,10 +375,7 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
     """GPU implementation of tsfresh.extract_features (extraction.py:30-190).  Returns the same
     pandas.DataFrame (float64, index = sorted ids, columns `{kind}__{calculator}[__{params}]`), or the
     list of (id, name, value) triples when pivot=False."""
-    if default_fc_parameters is None and kind_to_fc_parameters is None:
-        default_fc_parameters = ComprehensiveFCParameters()
-    elif default_fc_parameters is None and kind_to_fc_parameters is not None:
-        default_fc_parameters = {}
+    default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
     from .rolling import RolledTimeSeries
     if isinstance(timeseries_container, RolledTimeSeries):
         return _extract_rolled(timeseries_container, default_fc_parameters, kind_to_fc_parameters, impute_function,
@@ -383,43 +401,22 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
     if shared:
         plans, names = [], []
         for kind, _ids, sort_col, values, has_dt in frames:
-            fc = kind_to_fc_parameters[kind] if (kind_to_fc_parameters and kind in kind_to_fc_parameters) else default_fc_parameters
-            plan = Plan(fc, has_datetime_index=has_dt)
-            if show_warnings:
-                for name in plan.skipped:
-                    warnings.warn("{} requires the data to have a index of type {}. Results will "
-                                  "not be calculated".format(name, pd.DatetimeIndex))
+            plan, kind_names = _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters, has_dt, show_warnings)
             plans.append(plan)
-            names += [str(kind) + "__" + sfx for sfx in plan.suffixes]
+            names += kind_names
         if len(codes[0]) and all(p.n_cols > 0 for p in plans):
             dps = [_device_plan(ctx, p) for p in plans]
             times = frames[0][3].index.as_unit("ns").asi8 if any(p.needs_times for p in plans) else None
             flags_k = _lib.FLAG_IMPUTE if device_impute else 0
-            try:
+            with _nan_column(", ".join(str(f[3].name) for f in frames)):
                 uid, mat = _lib.extract_long_kinds(ctx, dps, codes[0], _sort_keys(frames[0][2]),
                                                    [f[3].to_numpy().astype(np.float32, copy=False) for f in frames], flags=flags_k,
                                                    times=times)
-            except ValueError as e:
-                if "contains NaN" in str(e):
-                    raise ValueError("Column must not contain NaN values: {}".format(
-                        ", ".join(str(f[3].name) for f in frames))) from None
-                raise
             blocks.append((names, uid, mat))
             frames, codes = [], []
             extract_flags = flags_k
     for (kind, _ids, sort_col, values, has_dt), id_codes in zip(frames, codes):
-        if kind_to_fc_parameters and kind in kind_to_fc_parameters:
-            fc = kind_to_fc_parameters[kind]
-        else:
-            fc = default_fc_parameters
-        value_name = values.name
-        kind = str(kind)
-        plan = Plan(fc, has_datetime_index=has_dt)
-        for name in plan.skipped:
-            if show_warnings:
-                warnings.warn("{} requires the data to have a index of type {}. Results will "
-                              "not be calculated".format(name, pd.DatetimeIndex))
-        names = [kind + "__" + s for s in plan.suffixes]
+        plan, names = _kind_plan(kind, default_fc_parameters, kind_to_fc_parameters, has_dt, show_warnings)
         if plan.n_cols == 0 or len(id_codes) == 0:
             uid = np.unique(id_codes)
             blocks.append((names, uid, np.empty((len(uid), 0))))
@@ -428,7 +425,7 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
         v32 = values.to_numpy().astype(np.float32, copy=False)
         # linear_trend_timewise regresses on the rows' DatetimeIndex (feature_calculators.py:2296-2299)
         times = values.index.as_unit("ns").asi8 if plan.needs_times else None
-        try:
+        with _nan_column(values.name):
             multi = None
             if len(gpus) > 1 and times is None and not extract_flags and len(id_codes) >= (1 << 20):
                 multi = _extract_long_multi(gpus, plan, id_codes, _sort_keys(sort_col), v32)
@@ -436,10 +433,6 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
                 uid, mat = multi
             else:
                 uid, mat = dp.extract_long(id_codes, _sort_keys(sort_col), v32, flags=extract_flags, times=times)
-        except ValueError as e:
-            if "contains NaN" in str(e):          # TSFX_E_NAN: the check of data.py:148-167, done on the device
-                raise ValueError("Column must not contain NaN values: {}".format(value_name)) from None
-            raise
         blocks.append((names, uid, mat))
 
     # ---- assemble (PartitionedTsData.pivot, data.py:86-121): union of ids, sorted, id dtype restored
@@ -474,10 +467,8 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
         result = result.sort_index()
     if impute_function is not None:
         if device_impute:
-            if not extract_flags and result.shape[0] and result.shape[1]:      # several kinds: one pass over the union
-                m = np.ascontiguousarray(result.to_numpy(dtype=np.float64))
-                ctx.impute(m, _lib.IMPUTE_RANGE)
-                result = pd.DataFrame(m, index=result.index, columns=result.columns, copy=False)
+            if not extract_flags:                     # several kinds: one pass over the union
+                result = _impute_on_device(ctx, result)
         else:
             impute_function(result)
     return result
