@@ -16,6 +16,13 @@
 #include "tsfx_common.cuh"
 #include "tsfx_kernels.h"
 
+// Builds for profiles/scripts/time_entropy_phases.py: -DTSFX_ENTROPY_SKIP=k leaves phase k of the rank-space kernel out
+// (1 load + moments, 2 the sorting network, 3 prefix table, 4 interval ends, 5 template counts), so the group's time
+// splits by phase.  Their results are wrong; the library build never sets it.
+#ifndef TSFX_ENTROPY_SKIP
+#define TSFX_ENTROPY_SKIP 0
+#endif
+
 namespace tsfx {
 
 // |x| as one integer AND on the high word (keeps the half-rate FP64 pipe for the subtractions and compares)
@@ -162,7 +169,11 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 4 ? 3 : 1)) k_entropy(Entrop
 // searches per (row, tolerance) with exactly the predicate numpy evaluates ( fl64(x_a - x_b) <= tau ), so the counts
 // are bit-identical to the bit-tile formulation above.  O(n^2 / 32) word operations + O(n log n) searches per
 // tolerance instead of O(n^2) float64 compares.
-// G warps work on one series (G = 1: warp per series; G > 1: the CTA is one series and shares the table).
+// G warps work on one series (G = 1: warp per series; G > 1: the CTA is one series and shares the table).  With one warp
+// per series (at most 256 samples) the sort runs in registers (warp_sort256), the table stores of a warp start on
+// distinct banks and the two 16-byte chunks of every table row with bit 2 set are swapped, so phase B's random-row loads
+// use all eight 16-byte bank groups.  Interval ends by merge path instead of the searches and the histogram were
+// measured slower there (DESIGN.md section 4).
 template <int G>
 __device__ __forceinline__ void gsync() { if (G == 1) __syncwarp(); else __syncthreads(); }
 
@@ -173,6 +184,43 @@ __device__ __forceinline__ unsigned f32_key(float f) {      // order-preserving;
 }
 __device__ __forceinline__ float key_f32(unsigned k) {
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// Bitonic sort of 256 64-bit keys, lane L holding positions 8L .. 8L + 7: strides below 8 inside the lane's registers,
+// the larger ones by shuffle.  The keys are unique, so the order is the one any sorting network gives.
+__device__ __forceinline__ void cmpx_regs(unsigned long long (&v)[8], int e, int f, bool up) {
+    const unsigned long long a = v[e], c = v[f];
+    if ((a > c) == up) { v[e] = c; v[f] = a; }
+}
+__device__ __forceinline__ void warp_sort256(unsigned long long (&v)[8], int lane) {
+#pragma unroll
+    for (int k = 2; k <= 8; k <<= 1) {                 // blocks of 8 inside the lane (direction from position 8L + e)
+#pragma unroll
+        for (int j = k >> 1; j > 0; j >>= 1) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (!(e & j)) cmpx_regs(v, e, e | j, ((8 * lane + e) & k) == 0);
+        }
+    }
+#pragma unroll 1
+    for (int k = 16; k <= 256; k <<= 1) {              // from here the direction is the lane's
+        const bool up = (lane & (k >> 3)) == 0;
+#pragma unroll 1
+        for (int jl = k >> 4; jl > 0; jl >>= 1) {      // strides 8 jl: partner lane ^ jl
+            const bool keep_min = up != ((lane & jl) != 0);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const unsigned long long o = __shfl_xor_sync(FULL, v[e], jl);
+                v[e] = keep_min ? (o < v[e] ? o : v[e]) : (o > v[e] ? o : v[e]);
+            }
+        }
+#pragma unroll
+        for (int j = 4; j > 0; j >>= 1) {
+#pragma unroll
+            for (int e = 0; e < 8; ++e)
+                if (!(e & j)) cmpx_regs(v, e, e | j, up);
+        }
+    }
 }
 
 struct RankLayout {            // byte offsets inside one series' working region
@@ -237,38 +285,71 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
         int64_t b; int n;
         if (A.R.begin) { b = A.R.begin[s]; n = A.R.len[s]; } else { b = s * (int64_t)A.R.dense_len; n = A.R.dense_len; }
         const float* src = A.R.values + b;
-        for (int i = tid; i < n; i += NTHR) xs[i] = __ldg(src + i);
-        gsync<G>();
-        const Moments M = moments(xs, n, nullptr, lane);          // identical in every warp of the group
+        Moments M;
+        if (TSFX_ENTROPY_SKIP == 1) {          // a hashed series in place of the load, a fixed sd in place of the moments
+            for (int i = tid; i < n; i += NTHR) xs[i] = (float)((unsigned)(i + s) * 2654435761u >> 8) * 0x1p-24f;
+            gsync<G>();
+            M.sd = 0.3;
+        } else {
+            for (int i = tid; i < n; i += NTHR) xs[i] = __ldg(src + i);
+            gsync<G>();
+            M = moments(xs, n, nullptr, lane);          // identical in every warp of the group
+        }
         int N2 = 32;
         while (N2 < n) N2 <<= 1;
-        for (int i = tid; i < N2; i += NTHR)
-            keys[i] = i < n ? (((unsigned long long)f32_key(xs[i]) << 32) | (unsigned)i) : ~0ull;
-        gsync<G>();
-        // ---- bitonic sort by value (payload: time index)
-        for (int k = 2; k <= N2; k <<= 1) {
-            for (int j = k >> 1; j > 0; j >>= 1) {
-                for (int t = tid; t < (N2 >> 1); t += NTHR) {
-                    const int i = 2 * t - (t & (j - 1));
-                    const int l = i + j;
-                    const unsigned long long a = keys[i], c = keys[l];
-                    const bool up = (i & k) == 0;
-                    if ((a > c) == up) { keys[i] = c; keys[l] = a; }
-                }
-                gsync<G>();
+        if constexpr (G == 1) {
+            // ---- sort by value (payload: time index) in registers, lane L holding positions 8L .. 8L + 7 (the launcher
+            // takes this path for series of at most 256 samples); sk, pi and rk are written once
+            unsigned long long v[8];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int i = 8 * lane + e;
+                v[e] = i < n ? (((unsigned long long)f32_key(xs[i]) << 32) | (unsigned)i) : ~0ull;
             }
-        }
-        // sorted keys (for the searches), rank <-> time maps.  keys alias T: read everything before T is built
-        const int per = (N2 + NTHR - 1) / NTHR;
-        for (int q = 0; q < per; ++q) {
-            const int a = tid + q * NTHR;
-            if (a < N2) {
-                const unsigned long long kv = keys[a];
-                sk[a] = (unsigned)(kv >> 32);              // 0xffffffff beyond n
-                if (a < n) {
-                    const unsigned idx = (unsigned)kv;
-                    pi[a] = (unsigned short)idx;
-                    rk[idx] = (unsigned short)a;
+            if (TSFX_ENTROPY_SKIP != 2) warp_sort256(v, lane);
+            unsigned kw[8], pk[4];
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const int a = 8 * lane + e;
+                const unsigned idx = (unsigned)v[e];
+                kw[e] = (unsigned)(v[e] >> 32);                        // 0xffffffff beyond n
+                if (e & 1) pk[e >> 1] |= (idx & 0xffffu) << 16; else pk[e >> 1] = idx & 0xffffu;
+                if (a < n) rk[idx] = (unsigned short)a;
+            }
+            if (8 * lane < N2) {                                       // N2 is a multiple of 32: whole 8-key runs
+                reinterpret_cast<uint4*>(sk)[2 * lane] = make_uint4(kw[0], kw[1], kw[2], kw[3]);
+                reinterpret_cast<uint4*>(sk)[2 * lane + 1] = make_uint4(kw[4], kw[5], kw[6], kw[7]);
+                reinterpret_cast<uint4*>(pi)[lane] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+            }
+        } else {
+            for (int i = tid; i < N2; i += NTHR)
+                keys[i] = i < n ? (((unsigned long long)f32_key(xs[i]) << 32) | (unsigned)i) : ~0ull;
+            gsync<G>();
+            // ---- bitonic sort by value (payload: time index)
+            for (int k = 2; k <= (TSFX_ENTROPY_SKIP == 2 ? 1 : N2); k <<= 1) {
+                for (int j = k >> 1; j > 0; j >>= 1) {
+                    for (int t = tid; t < (N2 >> 1); t += NTHR) {
+                        const int i = 2 * t - (t & (j - 1));
+                        const int l = i + j;
+                        const unsigned long long a = keys[i], c = keys[l];
+                        const bool up = (i & k) == 0;
+                        if ((a > c) == up) { keys[i] = c; keys[l] = a; }
+                    }
+                    gsync<G>();
+                }
+            }
+            // sorted keys (for the searches), rank <-> time maps.  keys alias T: read everything before T is built
+            const int per = (N2 + NTHR - 1) / NTHR;
+            for (int q = 0; q < per; ++q) {
+                const int a = tid + q * NTHR;
+                if (a < N2) {
+                    const unsigned long long kv = keys[a];
+                    sk[a] = (unsigned)(kv >> 32);              // 0xffffffff beyond n
+                    if (a < n) {
+                        const unsigned idx = (unsigned)kv;
+                        pi[a] = (unsigned short)idx;
+                        rk[idx] = (unsigned short)a;
+                    }
                 }
             }
         }
@@ -276,10 +357,16 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
         // ---- prefix table T[k][w], k = 0..n: bit j of T[k] = [rank(j) < k]
         const int W = (n + 31) >> 5;
         const int Wr = ((W + 3) >> 2) << 2;                 // the main loop reads whole 16-byte chunks
-        {
+        // one warp per series, rows of two 16-byte chunks: row k keeps its chunks swapped when bit 2 of k is set, so the
+        // chunk c of random rows spreads over all eight 16-byte bank groups (not the four of its parity)
+        const unsigned swz = (G == 1 && Wr == 8) ? 4u : 0u;
+        if (TSFX_ENTROPY_SKIP != 3) {
             int NC = NTHR / Wr;                              // k-chunks per word column
             if (NC < 1) NC = 1;
-            const int CH = (n + NC - 1) / NC;                // rows per chunk (the last chunk also writes row n)
+            int CH = (n + NC - 1) / NC;                      // rows per chunk (the last chunk also writes row n)
+            // one warp per series (NC * Wr = 32): CH = 1 mod NC puts the NC chunks' rows on distinct banks when the row
+            // stride is Wr words, so a store of the loop below is one wavefront instead of NC
+            if (G == 1) CH += (NC + 1 - CH % NC) % NC;
             const int items = NC * Wr;
             for (int it0 = (tid & ~31); it0 < items; it0 += NTHR) {      // warp-uniform trip count
                 unsigned init = 0u;
@@ -299,13 +386,12 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
                     int k1 = k0 + CH;
                     if (k1 > n) k1 = n;
                     unsigned cur = init;
-                    unsigned* col = T + w;
                     for (int k = k0; k < k1; ++k) {
-                        col[(size_t)k * RS] = cur;
+                        T[(size_t)k * RS + (w ^ (k & 4 ? swz : 0u))] = cur;
                         const unsigned p = pi[k];
                         if ((int)(p >> 5) == w) cur |= 1u << (p & 31);
                     }
-                    if (k1 == n) col[(size_t)n * RS] = cur;      // row n (every rank below n): written by the chunk(s) ending there
+                    if (k1 == n) T[(size_t)n * RS + (w ^ (n & 4 ? swz : 0u))] = cur;   // row n (every rank below n): written by the chunk(s) ending there
                 }
             }
         }
@@ -333,7 +419,9 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
             unsigned* lhq[2] = {lohi, lohi + L.lh_stride};
             for (int r = tid; r <= n; r += NTHR) cnt[r] = 0u;
             gsync<G>();
-            {
+            if (TSFX_ENTROPY_SKIP == 4) {
+                for (int r = tid; r < n; r += NTHR) { lhq[0][r] = r; lhq[1][r] = r; }
+            } else {
                 constexpr int U = 4;                                 // ranks per lane and tolerance in flight
                 for (int r0 = tid; r0 < n; r0 += U * NTHR) {
                     unsigned kL[2][U];
@@ -379,13 +467,23 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
                 }
             }
             gsync<G>();
-            {   // inclusive scan of the histograms by the whole group: thread t owns a contiguous run of ranks, warp scans by
+            if (TSFX_ENTROPY_SKIP == 4) {
+                for (int r = tid; r < n; r += NTHR) { lhq[0][r] = r | (r + 1) << 16; lhq[1][r] = r | (r + 1) << 16; }
+            } else {    // inclusive scan of the histograms by the whole group: thread t owns a contiguous run of ranks, warp scans by
                 // shuffle, warp totals through shared memory (with one warp per series the last step disappears)
                 const int run = (n + NTHR - 1) / NTHR;
                 const int b0 = tid * run;
+                // a whole run of 8 (one warp, n > 224) moves as two 16-byte words: lane-strided scalar accesses would hit
+                // every bank 8 times
+                const bool vec = G == 1 && run == 8 && b0 + 8 <= n;
                 unsigned v[8];
                 unsigned tot = 0u;
-                if (run <= 8) {         // the run lives in registers: one dependent shared-memory round trip, not one per rank
+                if (vec) {
+                    const uint4 c0 = reinterpret_cast<const uint4*>(cnt + b0)[0], c1 = reinterpret_cast<const uint4*>(cnt + b0)[1];
+                    v[0] = c0.x; v[1] = c0.y; v[2] = c0.z; v[3] = c0.w; v[4] = c1.x; v[5] = c1.y; v[6] = c1.z; v[7] = c1.w;
+#pragma unroll
+                    for (int k = 0; k < 8; ++k) { tot += v[k]; v[k] = tot; }
+                } else if (run <= 8) {  // the run lives in registers: one dependent shared-memory round trip, not one per rank
 #pragma unroll
                     for (int k = 0; k < 8; ++k) { const int r = b0 + k; v[k] = (k < run && r < n) ? cnt[r] : 0u; }
 #pragma unroll
@@ -403,7 +501,25 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
                     __syncthreads();
                     for (int w = 0; w < gw; ++w) off += wtot[w];
                 }
-                if (run <= 8) {
+                if (vec) {
+#pragma unroll
+                    for (int q = 0; q < 2; ++q) {
+                        if (q < nq) {
+                            uint4* p = reinterpret_cast<uint4*>(lhq[q] + b0);
+                            const bool sane = q == 0 ? sane0 : sane1;
+                            unsigned w[8];
+                            const uint4 l0 = p[0], l1 = p[1];
+                            w[0] = l0.x; w[1] = l0.y; w[2] = l0.z; w[3] = l0.w; w[4] = l1.x; w[5] = l1.y; w[6] = l1.z; w[7] = l1.w;
+#pragma unroll
+                            for (int k = 0; k < 8; ++k) {
+                                const unsigned acc = off + v[k];
+                                w[k] = sane ? (w[k] | (q == 0 ? acc << 16 : acc & 0xffff0000u)) : 0x00010001u;
+                            }
+                            p[0] = make_uint4(w[0], w[1], w[2], w[3]);
+                            p[1] = make_uint4(w[4], w[5], w[6], w[7]);
+                        }
+                    }
+                } else if (run <= 8) {
 #pragma unroll
                     for (int k = 0; k < 8; ++k) {
                         const int r = b0 + k;
@@ -457,8 +573,13 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
                     int c2[2] = {0, 0}, c3[2] = {0, 0};
                     if (NC > 0) {
                         uint4 hA[NC > 0 ? NC : 1], lA[NC > 0 ? NC : 1], hB[NC > 0 ? NC : 1], lB[NC > 0 ? NC : 1];
+                        // swapped chunks (swz, NC == 2 only): chunk c of row k at c ^ bit 2 of k
+                        const unsigned zhA = (lhA >> 18) & (swz >> 2), zlA = (lhA >> 2) & (swz >> 2);
+                        const unsigned zhB = (lhB >> 18) & (swz >> 2), zlB = (lhB >> 2) & (swz >> 2);
 #pragma unroll
-                        for (int c = 0; c < NC; ++c) { hA[c] = ThiA[c]; lA[c] = TloA[c]; hB[c] = ThiB[c]; lB[c] = TloB[c]; }
+                        for (int c = 0; c < NC; ++c) {
+                            hA[c] = ThiA[c ^ zhA]; lA[c] = TloA[c ^ zlA]; hB[c] = ThiB[c ^ zhB]; lB[c] = TloB[c ^ zlB];
+                        }
 #pragma unroll
                         for (int c = 0; c < NC; ++c) {
                             TSFX_RANK_STEP(0, hA[c].x & ~lA[c].x) TSFX_RANK_STEP(1, hB[c].x & ~lB[c].x)
@@ -483,7 +604,8 @@ __global__ void __launch_bounds__(G * SPC * 32, (G == 1 ? 4 : (G == 4 ? 4 : 1)))
                     }
                 }
             };
-            if (Wr == 8) sweep(std::integral_constant<int, 2>());
+            if (TSFX_ENTROPY_SKIP == 5) {}
+            else if (Wr == 8) sweep(std::integral_constant<int, 2>());
             else if (Wr == 4) sweep(std::integral_constant<int, 1>());
             else if (Wr == 12) sweep(std::integral_constant<int, 3>());
             else sweep(std::integral_constant<int, 0>());
@@ -524,7 +646,7 @@ cudaError_t launch_entropy(const EntropyArgs& A0, int max_len, cudaStream_t st, 
         const size_t s4 = lnk + (size_t)rank_layout(A.npad, 4, 1).bytes;
         const size_t s16 = lnk + (size_t)rank_layout(A.npad, 16, 1).bytes;
         const int64_t waves = grid_waves(16);
-        if (s1 <= 75 * 1024) {
+        if (A.npad <= 256 && s1 <= 75 * 1024) {         // the warp-per-series path sorts 256 keys in registers
             *variant = "entropy/rank-g1";
             const int ctas_per_sm = (int)std::min<size_t>(4, 227 * 1024 / (s1 + 1024));
             return launch_fixed(k_entropy_rank<1, 4>, 4 * 32, 4, s1, (int64_t)sm_count * ctas_per_sm * waves, A.R.n_series, st, A);
