@@ -261,6 +261,33 @@ int tsfx_extract_long_kinds(tsfx_ctx* ctx, const tsfx_plan* const* plans, const 
                             int32_t sort_key_is_f64, const float* const* values, int32_t n_kinds, int64_t n_rows,
                             int64_t** out_ids, double** out, int64_t* n_series_out, uint32_t flags);
 
+/* Long format with a KIND column (data.py:233-291 LongTsFrameAdapter): rows (ids[i], sort_keys[i], kind_codes[i],
+ * values[i]) in any order, all of them device pointers (TSFX_FLAG_DEVICE_PTRS is required).  The result has one row per
+ * id of ANY kind, ids ascending, and one column block per kind -- the frame PartitionedTsData.pivot builds (data.py:
+ * 86-121) -- so its row count is only known after grouping.  Extraction therefore takes two calls on the context:
+ *   tsfx_stage_long_stacked  partitions the rows by kind code (kind_codes int32, or int64 with kind_code_is_i64; NULL:
+ *                            every row is kind 0) with a stable counting sort, orders every kind's rows by (id, sort key)
+ *                            as tsfx_extract_long does (sort_keys NULL = keep row order; stable for equal keys), takes
+ *                            the union of the kinds' ids, synchronises the stream once and returns the union size
+ *                            in *n_ids_out, and per kind its row count and longest series (arrays of n_kinds entries,
+ *                            host).  row_time_ns (optional, int64 ns per row) follows the rows for linear_trend_timewise.
+ *                            TSFX_E_INVALID for a code outside 0 .. n_kinds-1 (1 <= n_kinds <= 64), TSFX_E_NAN for a
+ *                            NaN value or float64 sort key, TSFX_E_UNSUPPORTED for more than 2^31 - 4 098 rows.  The staged rows
+ *                            live in the context's working region until the next stage call.
+ *   tsfx_extract_staged      consumes what the last stage call staged: plans[k] is kind k's plan (may be NULL for a
+ *                            kind without rows, which contributes no columns).  Checks every kind's length limit
+ *                            (TSFX_E_TOO_LONG) before any kernel runs, then fills out ([n_ids x ld] row-major float64,
+ *                            device) with NaN where an id has no rows of a kind, writes each kind's columns at its
+ *                            column offset (blocks in kind order) and the union ids to out_ids (device).  ld >= the
+ *                            total column count; TSFX_FLAG_IMPUTE (needs ld == that count) imputes the matrix after.
+ *                            Asynchronous on the context's stream. */
+int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
+                            const float* values, const void* kind_codes, int32_t kind_code_is_i64, int32_t n_kinds,
+                            const int64_t* row_time_ns, int64_t n_rows, int64_t* n_ids_out, int64_t* rows_per_kind,
+                            int32_t* max_len_per_kind, uint32_t flags);
+int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* out_ids, double* out, int32_t ld,
+                        uint32_t flags);
+
 /* Page-locked host memory from the context's pool (freed blocks are cached: page-locking is slow). */
 void* tsfx_host_alloc(tsfx_ctx* ctx, size_t bytes);
 void tsfx_host_free(tsfx_ctx* ctx, void* p);

@@ -37,7 +37,7 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_extract_long", "tsfx_roll_windows", "tsfx_get_timings",
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
-           "tsfx_ctx_set_stream", "tsfx_set_out_ld"]
+           "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged"]
 
 
 def load():
@@ -86,6 +86,8 @@ def load():
         lib.tsfx_select_regression.argtypes = [vp, vp, i64, i32, vp, vp, u32]
         lib.tsfx_extract_long_kinds.argtypes = [vp, vp, vp, vp, i32, vp, i32, i64, ctypes.POINTER(vp), ctypes.POINTER(vp),
                                                 ctypes.POINTER(i64), u32]
+        lib.tsfx_stage_long_stacked.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, i64, ctypes.POINTER(i64), vp, vp, u32]
+        lib.tsfx_extract_staged.argtypes = [vp, vp, vp, vp, i32, u32]
         _lib = lib
         return lib
 
@@ -201,6 +203,26 @@ class Context:
                                       FLAG_ALL_MEDIANS if all_medians else 0)
             self.check(rc, "tsfx_impute")
         return stats
+
+    def stage_long_stacked(self, ids_ptr, sort_ptr, sort_is_f64, values_ptr, kind_ptr, kind_is_i64, n_kinds, times_ptr,
+                           n_rows):
+        """tsfx_stage_long_stacked on device rows (pointers as ints, 0 for an absent column): returns (number of union
+        ids, rows of every kind, longest series of every kind).  Synchronises the context's stream once."""
+        n_ids = ctypes.c_int64(0)
+        rows = np.zeros(n_kinds, dtype=np.int64)
+        max_len = np.zeros(n_kinds, dtype=np.int32)
+        rc = self.lib.tsfx_stage_long_stacked(self.h, ctypes.c_void_p(ids_ptr), ctypes.c_void_p(sort_ptr or None),
+                                              int(sort_is_f64), ctypes.c_void_p(values_ptr), ctypes.c_void_p(kind_ptr or None),
+                                              int(kind_is_i64), int(n_kinds), ctypes.c_void_p(times_ptr or None), int(n_rows),
+                                              ctypes.byref(n_ids), _ptr(rows), _ptr(max_len), FLAG_DEVICE_PTRS)
+        self.check(rc, "tsfx_stage_long_stacked")
+        return n_ids.value, rows, max_len
+
+    def extract_staged(self, device_plans, ids_ptr, out_ptr, ld, flags=0):
+        """tsfx_extract_staged: device_plans[k] is kind k's DevicePlan (None for a kind without rows)"""
+        plans = (ctypes.c_void_p * len(device_plans))(*[None if dp is None else dp.h for dp in device_plans])
+        rc = self.lib.tsfx_extract_staged(self.h, plans, ctypes.c_void_p(ids_ptr), ctypes.c_void_p(out_ptr), int(ld), flags)
+        self.check(rc, "tsfx_extract_staged")
 
     def impute_device(self, matrix_ptr, rows, cols, mode=IMPUTE_RANGE):
         rc = self.lib.tsfx_impute(self.h, ctypes.c_void_p(matrix_ptr), rows, cols, mode, None, FLAG_DEVICE_PTRS)

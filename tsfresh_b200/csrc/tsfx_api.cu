@@ -249,6 +249,7 @@ struct tsfx_ctx {
     const char* kernels[G_COUNT];         // variant each group of the last pass ran (tsfx_last_kernels)
     int n_kernels = 0;
     CsrWorkspace csr;
+    StackedWorkspace stacked;    // tsfx_stage_long_stacked: the staged rows the next tsfx_extract_staged consumes
     ImputeWorkspace imp;
     SelectWorkspace sel;
     DevBuf sel_x, sel_y, sel_out;
@@ -414,6 +415,7 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     ctx->values.release(); ctx->begin.release(); ctx->len.release(); ctx->out.release(); ctx->misc.release(); ctx->stage.release();
     ctx->times.release(); ctx->times_sorted.release(); ctx->kvals.release(); ctx->kvals_sorted.release();
     ctx->csr.release();
+    ctx->stacked.release();
     ctx->imp.release();
     ctx->sel.release();
     ctx->sel_x.release(); ctx->sel_y.release(); ctx->sel_out.release();
@@ -739,6 +741,16 @@ extern "C" int tsfx_set_row_times(tsfx_ctx* ctx, const int64_t* row_time_ns, int
     return TSFX_OK;
 }
 
+// TSFX_E_TOO_LONG when a series of max_len samples exceeds the limit of one of the plan's kernel groups
+static int check_lengths(tsfx_ctx* ctx, const tsfx_plan* P, int max_len) {
+    for (int g = 0; g < G_COUNT; ++g)
+        if (!P->host[g].empty() && max_len > group_max_len(g))
+            return fail(ctx, TSFX_E_TOO_LONG, std::string("series length ") + std::to_string(max_len) +
+                                                  " exceeds the shared-memory staging of kernel group " + kGroupNames[g] +
+                                                  " (limit " + std::to_string(group_max_len(g)) + " samples)");
+    return TSFX_OK;
+}
+
 static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int max_len, double* d_out, uint32_t flags, int ld = 0) {
     if (ld <= 0) ld = P->ncols;          // row stride of the caller's matrix
     const bool timing = (flags & TSFX_FLAG_TIMING) != 0;
@@ -748,11 +760,7 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
     if (R.n_series == 0) return TSFX_OK;
     const int staged = P->cum[G_COUNT];
     if (staged == 0) return TSFX_OK;
-    for (int g = 0; g < G_COUNT; ++g)          // every group's length limit before any group runs
-        if (!P->host[g].empty() && max_len > group_max_len(g))
-            return fail(ctx, TSFX_E_TOO_LONG, std::string("series length ") + std::to_string(max_len) +
-                                                  " exceeds the shared-memory staging of kernel group " + kGroupNames[g] +
-                                                  " (limit " + std::to_string(group_max_len(g)) + " samples)");
+    if (int rc = check_lengths(ctx, P, max_len)) return rc;      // every group's length limit before any group runs
     CK(ctx->stage.reserve((size_t)R.n_series * staged * sizeof(double)));
     CK(ctx->misc.reserve(max_len > 1024 ? ((size_t)1 << 30) : ((size_t)256 << 20)));      // global working regions for series too long for shared memory
     if (!P->host[G_SPECTRAL].empty()) {      // FFT twiddle table (filled once, on the main stream, before any fork)
@@ -1222,7 +1230,6 @@ static int stage_a_sort(tsfx_ctx* ctx, const LongIn& in, int max_blocks, bool ch
 }
 
 // the kinds of one call: plan, device value column (CSR order) and first output column of each
-#define TSFX_MAX_KINDS 64
 struct KindSet {
     int n = 1;
     const tsfx_plan* plan[TSFX_MAX_KINDS];
@@ -1450,6 +1457,112 @@ extern "C" int tsfx_extract_long_kinds(tsfx_ctx* ctx, const tsfx_plan* const* pl
     in.more = values + 1;
     in.n_kinds = n_kinds;
     return extract_long_pooled(ctx, plans, in, out_ids, out, n_series_out, flags);
+}
+
+// ------------------------------------------------------------------------------------------ stacked long format
+// the rows and their alignment gaps are counted in int (CUB scans)
+static const int64_t kMaxStackedRows = ((int64_t)1 << 31) - 2 - TSFX_MAX_KINDS * TSFX_STACK_ALIGN;
+extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
+                                       const float* values, const void* kind_codes, int32_t kind_code_is_i64, int32_t n_kinds,
+                                       const int64_t* row_time_ns, int64_t n_rows, int64_t* n_ids_out, int64_t* rows_per_kind,
+                                       int32_t* max_len_per_kind, uint32_t flags) {
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    S.valid = false;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (!(flags & TSFX_FLAG_DEVICE_PTRS)) return fail(ctx, TSFX_E_INVALID, "tsfx_stage_long_stacked takes device pointers");
+    if (n_kinds < 1 || n_kinds > TSFX_MAX_KINDS) return fail(ctx, TSFX_E_INVALID, "between 1 and 64 kinds per call");
+    if (n_rows < 0 || !n_ids_out || !rows_per_kind || !max_len_per_kind || (n_rows > 0 && (!ids || !values)))
+        return fail(ctx, TSFX_E_INVALID, "tsfx_stage_long_stacked: bad arguments");
+    if (n_rows > kMaxStackedRows) return fail(ctx, TSFX_E_UNSUPPORTED, "more than 2^31 - 4 098 rows in one call");
+    CK(cudaSetDevice(ctx->device));
+    *n_ids_out = 0;
+    for (int k = 0; k < n_kinds; ++k) { rows_per_kind[k] = 0; max_len_per_kind[k] = 0; }
+    S.n_kinds = n_kinds;
+    S.n_union = 0;
+    S.d_times = nullptr;
+    if (n_rows > 0) {
+        std::string msg;
+        int rc = stacked_stage(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values, kind_codes,
+                               kind_code_is_i64, n_kinds, row_time_ns, n_rows, ctx->stream, &msg);
+        if (rc) return fail(ctx, rc, msg);
+        CK(cudaStreamSynchronize(ctx->stream));
+        const StackedInfo& I = *S.h_info;
+        if (I.bad_kind) return fail(ctx, TSFX_E_INVALID, "a kind code is outside 0 .. " + std::to_string(n_kinds - 1));
+        if (I.nan_values) return nan_error(ctx);
+        if (I.nan_keys) return fail(ctx, TSFX_E_NAN, "the float64 sort keys contain NaN");
+        CK(S.keep_ids(ctx->csr.d_uid, I.n_union, ctx->stream));
+        S.n_union = I.n_union;
+        for (int k = 0; k < n_kinds; ++k) {
+            rows_per_kind[k] = I.kind_rows[k];
+            max_len_per_kind[k] = I.kind_max_len[k];
+        }
+    }
+    *n_ids_out = S.n_union;
+    S.valid = true;
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* out_ids, double* out, int32_t ld,
+                                   uint32_t flags) {
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (!S.valid) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: no rows staged (tsfx_stage_long_stacked)");
+    S.valid = false;
+    const int64_t U = S.n_union;
+    if (U == 0) return TSFX_OK;
+    if (!plans || !out_ids) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: bad arguments");
+    const StackedInfo& I = *S.h_info;
+    int col0[TSFX_MAX_KINDS], total = 0;
+    size_t block = 0;             // largest staging block of a kind that covers only some of the union rows
+    bool holes = false;
+    for (int k = 0; k < S.n_kinds; ++k) {
+        col0[k] = total;
+        if (I.kind_rows[k] == 0) continue;          // a kind without rows has no columns
+        const tsfx_plan* P = plans[k];
+        if (!P || P->ctx != ctx) return fail(ctx, TSFX_E_INVALID, "plan does not belong to this context");
+        total += P->ncols;
+        if (P->ncols == 0) continue;
+        if (int rc = check_lengths(ctx, P, I.kind_max_len[k])) return rc;
+        if (P->need_times && !S.d_times) return fail(ctx, TSFX_E_INVALID, "linear_trend_timewise needs the row timestamps");
+        const int64_t ns = I.kind_series[k + 1] - I.kind_series[k];
+        if (ns < U) { holes = true; block = std::max(block, (size_t)ns * P->ncols * sizeof(double)); }
+    }
+    if (total > 0 && !out) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: NULL out");
+    if (ld < total) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: row stride " + std::to_string(ld) + " < " + std::to_string(total) + " columns");
+    if (ld != total && (flags & TSFX_FLAG_IMPUTE)) return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_IMPUTE needs a contiguous result matrix");
+    CK(cudaSetDevice(ctx->device));
+    int launched = 0;
+    if (holes) {              // cells of an (id, kind) pair without rows stay NaN
+        CK(ctx->out.reserve(block));
+        CK(stacked_fill_nan(out, U, total, ld, ctx->stream));
+        launched += 1;
+    }
+    for (int k = 0; k < S.n_kinds; ++k) {
+        if (I.kind_rows[k] == 0 || plans[k]->ncols == 0) continue;
+        const tsfx_plan* P = plans[k];
+        const int64_t s0 = I.kind_series[k], ns = I.kind_series[k + 1] - s0;
+        SeriesRef R;
+        R.values = S.d_values; R.begin = S.d_begin + s0; R.len = S.d_len + s0; R.dense_len = 0; R.n_series = ns;
+        R.times = S.d_times;
+        // a kind with a series for every union row fills its columns in place; the others go through a staging block
+        // and are scattered to their union rows
+        double* dst = ns == U ? out + col0[k] : (double*)ctx->out.p;
+        int rc = run_groups(ctx, P, R, I.kind_max_len[k], dst, flags, ns == U ? ld : P->ncols);
+        if (rc) return rc;
+        launched += ctx->launches;
+        if (ns < U) {
+            CK(stacked_scatter(dst, ns, P->ncols, S.d_row + s0, out + col0[k], ld, ctx->stream));
+            launched += 1;
+        }
+    }
+    CK(cudaMemcpyAsync(out_ids, S.d_uid, (size_t)U * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
+    ctx->launches = launched;
+    if (flags & TSFX_FLAG_IMPUTE) return impute_after_extract(ctx, out, U, total);
+    return TSFX_OK;
 }
 
 extern "C" void* tsfx_host_alloc(tsfx_ctx* ctx, size_t bytes) {

@@ -265,6 +265,275 @@ int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys,
     return TSFX_OK;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// stacked long format (tsfx_csr.h)
+enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T_LEN, T_ROW, T_UID, T_INFO };
+
+cudaError_t StackedWorkspace::reserve(int slot, size_t bytes) {
+    if (bytes <= caps[slot]) return cudaSuccess;
+    if (bufs[slot]) cudaFree(bufs[slot]);
+    bufs[slot] = nullptr;
+    caps[slot] = 0;
+    cudaError_t e = cudaMalloc(&bufs[slot], bytes);
+    if (e == cudaSuccess) caps[slot] = bytes;
+    return e;
+}
+cudaError_t StackedWorkspace::keep_ids(const int64_t* d_src, int64_t n, cudaStream_t st) {
+    cudaError_t e = reserve(T_UID, std::max<size_t>((size_t)n * 8, 8));
+    if (e != cudaSuccess) return e;
+    d_uid = (int64_t*)bufs[T_UID];
+    return cudaMemcpyAsync(d_uid, d_src, (size_t)n * 8, cudaMemcpyDeviceToDevice, st);
+}
+void StackedWorkspace::release() {
+    for (int i = 0; i < 12; ++i) { if (bufs[i]) cudaFree(bufs[i]); bufs[i] = nullptr; caps[i] = 0; }
+    if (h_info) cudaFreeHost(h_info);
+    h_info = nullptr; d_info = nullptr;
+    d_values = nullptr; d_times = nullptr; d_begin = nullptr; d_len = nullptr; d_row = nullptr; d_uid = nullptr;
+    valid = false;
+}
+
+#define STACK_TILE 4096          // rows per CTA of the counting sort
+#define STACK_THREADS 256
+#define STACK_NO_KIND 0xFFu
+
+// Counting-sort histogram over the rows in CSR order: kind code of every row (STACK_NO_KIND when out of range), rows per
+// (kind, tile) into counts[k * n_tiles + tile]; NaN float64 sort keys (input order) are flagged on the way.
+__global__ void __launch_bounds__(STACK_THREADS) k_stack_count(const uint32_t* __restrict__ perm, const void* kinds, int kinds_i64,
+                                                               int n_kinds, const uint64_t* __restrict__ keys_f64, int64_t n,
+                                                               uint8_t* __restrict__ code, int* __restrict__ counts, StackedInfo* info) {
+    __shared__ int hist[TSFX_MAX_KINDS];
+    for (int k = threadIdx.x; k < TSFX_MAX_KINDS; k += blockDim.x) hist[k] = 0;
+    __syncthreads();
+    const int64_t lo = (int64_t)blockIdx.x * STACK_TILE, hi = min(lo + STACK_TILE, n);
+    int bad = 0, nan = 0;
+    for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+        const uint32_t src = perm[i];
+        int64_t c = 0;
+        if (kinds) c = kinds_i64 ? ((const int64_t*)kinds)[src] : (int64_t)((const int32_t*)kinds)[src];
+        const bool ok = c >= 0 && c < n_kinds;
+        code[i] = ok ? (uint8_t)c : (uint8_t)STACK_NO_KIND;
+        if (ok) atomicAdd(&hist[c], 1);
+        bad |= !ok;
+        if (keys_f64) { const double v = __longlong_as_double((long long)keys_f64[i]); nan |= v != v; }
+    }
+    if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(&info->bad_kind, 1);
+    if (__any_sync(0xffffffffu, nan) && (threadIdx.x & 31) == 0) atomicOr(&info->nan_keys, 1);
+    __syncthreads();
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) counts[(int64_t)k * gridDim.x + blockIdx.x] = hist[k];
+}
+
+// Stable scatter of the counting sort: each tile walks its rows in order, 256 at a time; a row's destination is its
+// kind's running base in this tile + the rows of that kind in earlier warps of the step + its rank among its warp's
+// rows of the same kind (__match_any_sync).  Gathers the value (already in CSR order), the union row and the time.
+__global__ void __launch_bounds__(STACK_THREADS) k_stack_scatter(const uint8_t* __restrict__ code, const int* __restrict__ offs,
+                                                                 int n_kinds, int64_t n, const float* __restrict__ vals,
+                                                                 const int32_t* __restrict__ urow, const int64_t* __restrict__ times,
+                                                                 const uint32_t* __restrict__ perm, const StackedInfo* info,
+                                                                 float* __restrict__ out_vals, int32_t* __restrict__ out_row,
+                                                                 int64_t* __restrict__ out_times) {
+    constexpr int W = STACK_THREADS / 32;
+    __shared__ int64_t base[TSFX_MAX_KINDS];
+    __shared__ int cnt[W][TSFX_MAX_KINDS];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x)        // the scan packs the kinds; their starts are aligned
+        base[k] = offs[(int64_t)k * gridDim.x + blockIdx.x] - offs[(int64_t)k * gridDim.x] + info->kind_row[k];
+    const int64_t lo = (int64_t)blockIdx.x * STACK_TILE, hi = min(lo + STACK_TILE, n);
+    for (int64_t c0 = lo; c0 < hi; c0 += STACK_THREADS) {
+        for (int j = threadIdx.x; j < W * TSFX_MAX_KINDS; j += blockDim.x) (&cnt[0][0])[j] = 0;
+        __syncthreads();
+        const int64_t i = c0 + threadIdx.x;
+        const unsigned k = i < hi ? code[i] : STACK_NO_KIND;
+        const unsigned peers = __match_any_sync(0xffffffffu, k);
+        const int rank = __popc(peers & ((1u << lane) - 1));
+        if (k != STACK_NO_KIND && rank == 0) cnt[warp][k] = __popc(peers);
+        __syncthreads();
+        if (k != STACK_NO_KIND) {
+            int64_t dst = base[k] + rank;
+            for (int w = 0; w < warp; ++w) dst += cnt[w][k];
+            out_vals[dst] = vals[i];
+            out_row[dst] = urow[i];
+            if (times) out_times[dst] = times[perm[i]];
+        }
+        __syncthreads();
+        for (int kk = threadIdx.x; kk < n_kinds; kk += blockDim.x) {
+            int add = 0;
+            for (int w = 0; w < W; ++w) add += cnt[w][kk];
+            base[kk] += add;
+        }
+        __syncthreads();
+    }
+}
+
+// rows and aligned first row of every kind
+__global__ void k_stack_kind_rows(const int* __restrict__ offs, int n_kinds, int n_tiles, StackedInfo* info) {
+    int64_t at = 0;
+    for (int k = 0; k < n_kinds; ++k) {
+        const int64_t rows = offs[(int64_t)(k + 1) * n_tiles] - offs[(int64_t)k * n_tiles];
+        info->kind_row[k] = at;
+        info->kind_rows[k] = rows;
+        at += (rows + TSFX_STACK_ALIGN - 1) / TSFX_STACK_ALIGN * TSFX_STACK_ALIGN;
+    }
+    info->kind_row[n_kinds] = at;
+}
+
+// kind whose aligned row range holds partitioned row j (the last of kinds that start at the same row is the only one
+// that can have rows)
+__device__ __forceinline__ int kind_at(const StackedInfo* info, int n_kinds, int64_t j) {
+    int lo = 0, hi = n_kinds;
+    while (hi - lo > 1) { const int m = (lo + hi) >> 1; if (info->kind_row[m] <= j) lo = m; else hi = m; }
+    return lo;
+}
+
+// 1 where row i of the sorted ids starts a new id (row 0 excluded): the inclusive scan is the union row of every row
+struct IdChange {
+    const int64_t* ids;
+    __device__ int operator()(int64_t i) const { return i > 0 && ids[i] != ids[i - 1]; }
+};
+
+// 1 where partitioned row j starts a series: the first row of a kind, or a new union row (0 in the alignment gaps)
+struct SeriesStart {
+    const int32_t* row;
+    const StackedInfo* info;
+    int n_kinds;
+    __device__ int operator()(int64_t j) const {
+        if (j >= info->kind_row[n_kinds]) return 0;
+        const int k = kind_at(info, n_kinds, j);
+        if (j >= info->kind_row[k] + info->kind_rows[k]) return 0;
+        return j == info->kind_row[k] || row[j] != row[j - 1];
+    }
+};
+
+__global__ void k_stack_series(const int32_t* __restrict__ sidx, SeriesStart start, int64_t n, int64_t* __restrict__ begin,
+                               int32_t* __restrict__ series_row) {
+    int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; j < n; j += stride)
+        if (start(j)) { const int32_t s = sidx[j]; begin[s] = j; series_row[s] = start.row[j]; }
+}
+
+// series lengths, each kind's first series and longest series
+__global__ void k_stack_lengths(const int32_t* __restrict__ sidx, int64_t n, int n_kinds, const int64_t* __restrict__ begin,
+                                int32_t* __restrict__ len, StackedInfo* info) {
+    __shared__ int mx[TSFX_MAX_KINDS];
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) mx[k] = 0;
+    __syncthreads();
+    const int64_t ns = sidx[n];
+    if (blockIdx.x == 0)
+        for (int k = threadIdx.x; k <= n_kinds; k += blockDim.x) info->kind_series[k] = sidx[info->kind_row[k]];
+    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; s < ns; s += stride) {
+        const int64_t b = begin[s];
+        const int k = kind_at(info, n_kinds, b);
+        int64_t e = info->kind_row[k] + info->kind_rows[k];
+        if (s + 1 < ns) e = min(e, begin[s + 1]);
+        const int32_t l = (int32_t)(e - b);
+        len[s] = l;
+        atomicMax(&mx[k], l);
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
+}
+
+__global__ void k_stack_finish(const CsrInfo* csr, StackedInfo* info) {
+    info->n_union = csr->n_series;
+    info->nan_values = csr->has_nan;
+}
+
+int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
+                  const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
+                  int64_t n, cudaStream_t st, std::string* msg) {
+    S.valid = false;
+    S.n_kinds = n_kinds;
+    if (!S.h_info) CKE(cudaHostAlloc((void**)&S.h_info, sizeof(StackedInfo), cudaHostAllocDefault), "alloc info");
+    CKE(S.reserve(T_INFO, sizeof(StackedInfo)), "alloc info");
+    S.d_info = (StackedInfo*)S.bufs[T_INFO];
+    CKE(cudaMemsetAsync(S.d_info, 0, sizeof(StackedInfo), st), "memset info");
+    // stage (a) over every row: (id, sort key) order, union of the ids, NaN scan of the values
+    int rc = csr_sort_pass(W, d_ids, d_keys, keys_f64, d_values, n, n, 1, true, st, msg);
+    if (rc) return rc;
+    const int n_tiles = (int)((n + STACK_TILE - 1) / STACK_TILE);
+    const int64_t n_pad = n + (int64_t)n_kinds * TSFX_STACK_ALIGN;       // partitioned rows and alignment gaps
+    const size_t n_counts = (size_t)n_kinds * n_tiles + 1;
+    CKE(S.reserve(T_CODE, n), "alloc codes");
+    CKE(S.reserve(T_UROW, (size_t)(n_pad + 1) * 4), "alloc rows");
+    CKE(S.reserve(T_COUNTS, n_counts * 4), "alloc counts");
+    CKE(S.reserve(T_VALS, (size_t)n_pad * 4), "alloc values");
+    CKE(S.reserve(T_SROW, (size_t)n_pad * 4), "alloc rows");
+    CKE(S.reserve(T_BEGIN, (size_t)n * 8), "alloc begin");
+    CKE(S.reserve(T_LEN, (size_t)n * 4), "alloc len");
+    CKE(S.reserve(T_ROW, (size_t)n * 4), "alloc map");
+    if (d_times) CKE(S.reserve(T_TIMES, (size_t)n_pad * 8), "alloc times");
+    uint8_t* code = (uint8_t*)S.bufs[T_CODE];
+    int32_t* urow = (int32_t*)S.bufs[T_UROW];      // union row of every CSR row; later the series index of every staged row
+    int* counts = (int*)S.bufs[T_COUNTS];
+    int32_t* srow = (int32_t*)S.bufs[T_SROW];
+    S.d_values = (float*)S.bufs[T_VALS];
+    S.d_times = d_times ? (int64_t*)S.bufs[T_TIMES] : nullptr;
+    S.d_begin = (int64_t*)S.bufs[T_BEGIN];
+    S.d_len = (int32_t*)S.bufs[T_LEN];
+    S.d_row = (int32_t*)S.bufs[T_ROW];
+    const int64_t* ids_sorted = (const int64_t*)W.bufs[S_IDS_SORTED];
+    thrust::counting_iterator<int64_t> rows(0);
+    size_t tb1 = 0, tb2 = 0, tb3 = 0;
+    auto id_change = thrust::make_transform_iterator(rows, IdChange{ids_sorted});
+    SeriesStart start{srow, S.d_info, n_kinds};
+    auto series_start = thrust::make_transform_iterator(rows, start);
+    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb1, id_change, urow, (int)n, st), "scan size");
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb2, counts, counts, (int)n_counts, st), "scan size");
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb3, series_start, urow, (int)(n_pad + 1), st), "scan size");
+    const size_t tb = std::max(tb1, std::max(tb2, tb3));
+    CKE(S.reserve(T_TEMP, tb), "alloc temp");
+    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb1, id_change, urow, (int)n, st), "union rows");
+    k_stack_count<<<n_tiles, STACK_THREADS, 0, st>>>(W.d_perm, d_kinds, kinds_i64, n_kinds, keys_f64 ? d_keys : nullptr, n,
+                                                     code, counts, S.d_info);
+    CKE(cudaGetLastError(), "kind count kernel");
+    CKE(cudaMemsetAsync(counts + n_counts - 1, 0, 4, st), "memset counts");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb2, counts, counts, (int)n_counts, st), "kind offsets");
+    k_stack_kind_rows<<<1, 1, 0, st>>>(counts, n_kinds, n_tiles, S.d_info);
+    k_stack_scatter<<<n_tiles, STACK_THREADS, 0, st>>>(code, counts, n_kinds, n, W.d_values, urow, d_times, W.d_perm,
+                                                       S.d_info, S.d_values, srow, S.d_times);
+    CKE(cudaGetLastError(), "kind scatter kernel");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb3, series_start, urow, (int)(n_pad + 1), st), "series index");
+    k_stack_series<<<grid_for(n_pad, 256), 256, 0, st>>>(urow, start, n_pad, S.d_begin, S.d_row);
+    k_stack_lengths<<<grid_for(n / 4 + 1, 256), 256, 0, st>>>(urow, n_pad, n_kinds, S.d_begin, S.d_len, S.d_info);
+    k_stack_finish<<<1, 1, 0, st>>>(W.d_info, S.d_info);
+    CKE(cudaGetLastError(), "series kernels");
+    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
+    return TSFX_OK;
+}
+
+__global__ void k_fill_nan(double* __restrict__ out, int64_t n_rows, int n_cols, int ld) {
+    int64_t e = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x, total = n_rows * n_cols;
+    for (; e < total; e += stride) out[(e / n_cols) * ld + e % n_cols] = __longlong_as_double(0x7ff8000000000000LL);
+}
+
+cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cudaStream_t st) {
+    if (n_rows <= 0 || n_cols <= 0) return cudaSuccess;
+    k_fill_nan<<<grid_for(n_rows * n_cols, 256), 256, 0, st>>>(out, n_rows, n_cols, ld);
+    return cudaGetLastError();
+}
+
+__global__ void k_scatter_rows(const double* __restrict__ block, int64_t n_series, int n_cols, const int32_t* __restrict__ row,
+                               double* __restrict__ out, int ld) {
+    const int lane = threadIdx.x & 31;
+    int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (; s < n_series; s += n_warps) {
+        const double* src = block + (size_t)s * n_cols;
+        double* dst = out + (size_t)row[s] * ld;
+        for (int c = lane; c < n_cols; c += 32) __stcs(dst + c, __ldcs(src + c));
+    }
+}
+
+cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, const int32_t* row, double* out, int ld,
+                            cudaStream_t st) {
+    if (n_series <= 0 || n_cols <= 0) return cudaSuccess;
+    k_scatter_rows<<<grid_for(n_series * 32, 256), 256, 0, st>>>(block, n_series, n_cols, row, out, ld);
+    return cudaGetLastError();
+}
+
 int csr_max_len(CsrWorkspace& W, const int32_t* d_len, int64_t n, cudaStream_t st, int* out) {
     std::string* msg = nullptr;
     CKE(W.reserve(S_FLAG, 64), "alloc");

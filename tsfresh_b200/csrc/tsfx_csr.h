@@ -76,6 +76,66 @@ int csr_max_len(CsrWorkspace& W, const int32_t* d_len, int64_t n, cudaStream_t s
 // NaN scan of a device float array; result lands in d_info->has_nan (async)
 void csr_check_nan(CsrWorkspace& W, const float* d_values, int64_t n, cudaStream_t st);
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Stacked long format: rows (id, sort key, kind code, value[, time]) in any order, several kinds in one frame
+// (data.py:233-291 LongTsFrameAdapter, whose pivot makes one row per id of ANY kind, data.py:86-121).
+//
+// One csr_sort_pass over all rows orders them by (id, sort key) and yields the union of the ids of every kind as its
+// unique ids.  A stable counting sort by kind code then partitions the rows in that order, so each kind's rows land
+// contiguous and still ordered by (id, sort key), each carrying the union row of its id.  Series start where the union
+// row or the kind changes; every series keeps (begin, len) into the partitioned values and the union row it fills.
+// Every kind's rows start at a multiple of TSFX_STACK_ALIGN rows: its series then have the alignment they have when the
+// kind is extracted on its own, and kernels whose summation order follows the alignment of the loads (k_moments) give
+// the same bits.
+#define TSFX_MAX_KINDS 64
+#define TSFX_STACK_ALIGN 64
+
+struct StackedInfo {              // written by the device, read once by the host
+    int32_t bad_kind;             // a kind code outside 0 .. n_kinds-1
+    int32_t nan_values;
+    int32_t nan_keys;             // a float64 sort key is NaN
+    int32_t pad;
+    int64_t n_union;              // distinct ids over all kinds
+    int64_t kind_row[TSFX_MAX_KINDS + 1];      // kind k's rows are [kind_row[k], + kind_rows[k]) of the partitioned arrays
+    int64_t kind_rows[TSFX_MAX_KINDS];
+    int64_t kind_series[TSFX_MAX_KINDS + 1];   // kind k's series are [kind_series[k], kind_series[k+1])
+    int32_t kind_max_len[TSFX_MAX_KINDS];
+};
+
+struct StackedWorkspace {
+    // the staged input: partitioned rows and per-series views (device), and what the host learnt about them
+    float* d_values = nullptr;    // row values, kind-major, (id, sort key) order inside a kind
+    int64_t* d_times = nullptr;   // row timestamps in the same order (nullptr: none were given)
+    int64_t* d_begin = nullptr;   // series s = d_values[d_begin[s] .. + d_len[s])
+    int32_t* d_len = nullptr;
+    int32_t* d_row = nullptr;     // union row of series s
+    int64_t* d_uid = nullptr;     // union ids, ascending (keep_ids)
+    StackedInfo* h_info = nullptr;   // pinned
+    StackedInfo* d_info = nullptr;
+    int n_kinds = 0;
+    int64_t n_union = 0;
+    bool valid = false;           // staged and not yet consumed
+    void* bufs[12] = {nullptr};
+    size_t caps[12] = {0};
+    cudaError_t reserve(int slot, size_t bytes);
+    cudaError_t keep_ids(const int64_t* d_src, int64_t n, cudaStream_t st);   // d_uid = a copy of n union ids
+    void release();
+};
+
+// Stages n_rows device rows (ids, sort keys (nullptr: input order), float32 values, kind codes (int32 / int64; nullptr:
+// every row is kind 0), optional int64 row times) into S, then copies S.d_info to S.h_info.  Asynchronous: the caller
+// synchronises and checks the flags before it relies on the sizes.  Uses W's sort buffers as scratch.
+int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
+                  const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
+                  int64_t n_rows, cudaStream_t st, std::string* msg);
+
+// out[r * ld + c] = NaN for r < n_rows, c < n_cols
+cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cudaStream_t st);
+
+// out[row[s] * ld + c] = block[s * n_cols + c] for s < n_series, c < n_cols (one warp per row)
+cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, const int32_t* row, double* out, int ld,
+                            cudaStream_t st);
+
 // Checked pass over caller-supplied device views (TSFX_FLAG_CHECK_DEVICE_INPUT), one launch: the longest series into
 // d_info->max_len, the first view with len < 1, begin < 0 or begin + len > n_values into d_info->bad_view_rev, and a NaN
 // among the values of the valid views into d_info->has_nan (async; d_info zeroed by the caller)

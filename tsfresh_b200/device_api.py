@@ -8,6 +8,13 @@ device and blocks the host once per kind, for the checked pass (include/tsfx.h, 
 measures the longest series and rejects invalid views and NaN values before any kernel group sees the input.
 Columns are named and ordered as `extract_features` names them for the equivalent wide frame (one value column per
 kind, no DatetimeIndex, so linear_trend_timewise is skipped); rows follow the input order.
+
+    X, row_ids, columns = extract_features_long_device(ids, values, sort, kind, kinds=[...])   # long format
+
+takes one tensor per column of a long frame, rows in any order, and returns what extract_features returns for that frame
+with column_kind: one row per id of any kind (ids ascending), one column block per kind.  Its row count is only known
+after the rows are grouped, so the library stages the rows first (tsfx_stage_long_stacked, one host synchronisation)
+and torch then allocates the result that the extraction (tsfx_extract_staged) fills.
 """
 import numpy as np
 import pandas as pd
@@ -155,3 +162,112 @@ def extract_features_device(values, begin=None, length=None, *, default_fc_param
         impute_function(df)
         X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
     return X, columns
+
+
+def _long_layout(ids, values, sort, kind, kinds, times):
+    """(number of rows, kind names) of long-format row tensors from their shapes and dtypes alone (no device needed)."""
+    import torch
+    columns = (("ids", ids), ("values", values), ("sort", sort), ("kind", kind), ("times", times))
+    for name, t in columns:
+        if t is None and name in ("ids", "values"):
+            raise TypeError("%s must be a torch.Tensor, not None" % name)
+        if t is None:
+            continue
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, not %s" % (name, type(t).__name__))
+        if t.ndim != 1:
+            raise ValueError("%s must be 1-D, got shape %s" % (name, tuple(t.shape)))
+    if ids.dtype != torch.int64:
+        raise TypeError("ids must be int64, not %s" % ids.dtype)
+    if values.dtype not in (torch.float32, torch.float64, torch.float16, torch.bfloat16):
+        raise TypeError("values must be float32, float64, float16 or bfloat16, not %s" % values.dtype)
+    if sort is not None and sort.dtype not in (torch.int64, torch.float64):
+        raise TypeError("sort must be int64 or float64, not %s" % sort.dtype)
+    if kind is not None and kind.dtype not in (torch.int32, torch.int64):
+        raise TypeError("kind must be int32 or int64, not %s" % kind.dtype)
+    if times is not None and times.dtype != torch.int64:
+        raise TypeError("times must be int64 nanoseconds, not %s" % times.dtype)
+    n = ids.shape[0]
+    for name, t in columns[1:]:
+        if t is not None and t.shape[0] != n:
+            raise ValueError("%s has %d rows, ids %d" % (name, t.shape[0], n))
+    if n > (1 << 31) - 2 - 64 * 64:
+        raise ValueError("%d rows: at most 2^31 - 4 098 in one call" % n)
+    if kind is None:
+        kinds = ["value"] if kinds is None else list(kinds)
+        if len(kinds) != 1:
+            raise ValueError("without kind codes there is one kind, %d named" % len(kinds))
+    else:
+        if kinds is None:
+            raise ValueError("kinds must name the kinds that the codes 0 .. K-1 of kind stand for")
+        kinds = list(kinds)
+        if not 1 <= len(kinds) <= 64:
+            raise ValueError("between 1 and 64 kinds, %d named" % len(kinds))
+    if len(set(map(str, kinds))) != len(kinds):
+        raise ValueError("kinds must have distinct names: %r" % (kinds,))
+    _check_colname(*kinds)
+    return n, kinds
+
+
+def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=None, times=None, default_fc_parameters=None,
+                                 kind_to_fc_parameters=None, impute_function=None):
+    """Extracts features from long-format rows held in CUDA tensors into a CUDA tensor.
+
+    ids (int64), values, sort, kind and times are 1-D CUDA tensors with one entry per row, rows in any order.
+    values: float32 is read in place; float64, float16 and bfloat16 are rounded to float32 on the device.
+    sort: int64 or float64 sort keys (None: rows keep their input order); equal keys keep their input order.
+    kind: int32 or int64 codes 0 .. K-1 of the kinds that `kinds` names (None: one kind, named "value").
+    times: int64 nanosecond timestamp of every row; given, linear_trend_timewise is computed as extract_features computes
+    it for a frame with that DatetimeIndex.
+    default_fc_parameters / kind_to_fc_parameters / impute_function: as extract_features_device.
+
+    Returns (X, row_ids, columns), what extract_features returns for the equivalent frame with column_kind: row_ids
+    (int64, CUDA) is the ascending union of the ids of every kind, X float64 [len(row_ids), len(columns)] on values'
+    device, one column block per kind in code order, NaN where an id has no rows of a kind; a kind without rows has no
+    columns.  Runs on torch's current stream and blocks the host once, to learn the number of ids.  Raises ValueError for
+    NaN values or sort keys, kind codes out of range and series longer than their kind's plan allows, before any feature
+    kernel runs."""
+    import torch
+    n, kinds = _long_layout(ids, values, sort, kind, kinds, times)
+    default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
+    plans = [_kind_plan(k, default_fc_parameters, kind_to_fc_parameters, has_datetime_index=times is not None)
+             for k in kinds]
+    dev = values.device
+    if dev.type != "cuda":
+        raise ValueError("values must be a CUDA tensor, got one on %s" % dev)
+    for name, t in (("ids", ids), ("sort", sort), ("kind", kind), ("times", times)):
+        if t is not None and t.device != dev:
+            raise ValueError("%s is on %s, values on %s" % (name, t.device, dev))
+    mode = _lib.IMPUTE_RANGE if impute_function is impute else _lib.IMPUTE_ZERO if impute_function is impute_dataframe_zero else None
+    with torch.cuda.device(dev):
+        v = values.contiguous() if values.dtype == torch.float32 else values.to(torch.float32).contiguous()
+        i = ids.contiguous()
+        s = None if sort is None else sort.contiguous()
+        k = None if kind is None else kind.contiguous()
+        t = None if times is None else times.contiguous()
+        ctx = get_context(dev.index)
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        with ctx.lock:
+            ctx.set_stream(stream or _lib.STREAM_LEGACY)
+            try:
+                n_ids, rows, _ = ctx.stage_long_stacked(
+                    i.data_ptr(), 0 if s is None else s.data_ptr(), s is not None and s.dtype == torch.float64,
+                    v.data_ptr(), 0 if k is None else k.data_ptr(), k is not None and k.dtype == torch.int64, len(kinds),
+                    0 if t is None else t.data_ptr(), n)
+                present = [c for c in range(len(kinds)) if rows[c] > 0]
+                columns = [name for c in present for name in plans[c][1]]
+                width = len(columns)
+                X = torch.empty((n_ids, width), dtype=torch.float64, device=dev)
+                row_ids = torch.empty(n_ids, dtype=torch.int64, device=dev)
+                dps = [_device_plan(ctx, plans[c][0]) if rows[c] > 0 else None for c in range(len(kinds))]
+                ctx.extract_staged(dps, row_ids.data_ptr(), X.data_ptr(), width,
+                                   _lib.FLAG_IMPUTE if mode == _lib.IMPUTE_RANGE else 0)
+                if mode == _lib.IMPUTE_ZERO and n_ids and width:
+                    ctx.impute_device(X.data_ptr(), n_ids, width, mode)
+            finally:
+                ctx.set_stream(None)
+    if impute_function is not None and mode is None:
+        df = pd.DataFrame(X.cpu().numpy(), columns=columns)
+        impute_function(df)
+        X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
+    return X, row_ids, columns
