@@ -15,6 +15,7 @@
 
 #include "tsfx_common.cuh"
 #include "tsfx_kernels.h"
+#include "tsfx_warp_sort.cuh"
 
 // Builds for profiles/scripts/time_entropy_phases.py: -DTSFX_ENTROPY_SKIP=k leaves phase k of the rank-space kernel out
 // (1 load + moments, 2 the sorting network, 3 prefix table, 4 interval ends, 5 template counts), so the group's time
@@ -184,43 +185,6 @@ __device__ __forceinline__ unsigned f32_key(float f) {      // order-preserving;
 }
 __device__ __forceinline__ float key_f32(unsigned k) {
     return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-// Bitonic sort of 256 64-bit keys, lane L holding positions 8L .. 8L + 7: strides below 8 inside the lane's registers,
-// the larger ones by shuffle.  The keys are unique, so the order is the one any sorting network gives.
-__device__ __forceinline__ void cmpx_regs(unsigned long long (&v)[8], int e, int f, bool up) {
-    const unsigned long long a = v[e], c = v[f];
-    if ((a > c) == up) { v[e] = c; v[f] = a; }
-}
-__device__ __forceinline__ void warp_sort256(unsigned long long (&v)[8], int lane) {
-#pragma unroll
-    for (int k = 2; k <= 8; k <<= 1) {                 // blocks of 8 inside the lane (direction from position 8L + e)
-#pragma unroll
-        for (int j = k >> 1; j > 0; j >>= 1) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if (!(e & j)) cmpx_regs(v, e, e | j, ((8 * lane + e) & k) == 0);
-        }
-    }
-#pragma unroll 1
-    for (int k = 16; k <= 256; k <<= 1) {              // from here the direction is the lane's
-        const bool up = (lane & (k >> 3)) == 0;
-#pragma unroll 1
-        for (int jl = k >> 4; jl > 0; jl >>= 1) {      // strides 8 jl: partner lane ^ jl
-            const bool keep_min = up != ((lane & jl) != 0);
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const unsigned long long o = __shfl_xor_sync(FULL, v[e], jl);
-                v[e] = keep_min ? (o < v[e] ? o : v[e]) : (o > v[e] ? o : v[e]);
-            }
-        }
-#pragma unroll
-        for (int j = 4; j > 0; j >>= 1) {
-#pragma unroll
-            for (int e = 0; e < 8; ++e)
-                if (!(e & j)) cmpx_regs(v, e, e | j, up);
-        }
-    }
 }
 
 struct RankLayout {            // byte offsets inside one series' working region
