@@ -62,6 +62,8 @@ extern "C" {
                                   * [0, n_values) with len >= 1 (else TSFX_E_INVALID), and no NaN among the values the
                                   * series cover (else TSFX_E_NAN).  No kernel group runs on input that fails the pass,
                                   * so tsfx_last_launch_count is 0 after such an error. */
+#define TSFX_FLAG_KEEP_SORT_KEYS 64u /* tsfx_stage_long_stacked: keep every staged row's sort key, which tsfx_roll_staged
+                                  * names its windows by (without the flag the call does no extra work) */
 
 /* tsfx_impute modes (tsfresh/utilities/dataframe_functions.py) */
 #define TSFX_IMPUTE_RANGE 0      /* impute :49-78: +inf -> max, -inf -> min, NaN -> median of the finite values */
@@ -287,6 +289,29 @@ int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const void* sort_
                             int32_t* max_len_per_kind, uint32_t flags);
 int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* out_ids, double* out, int32_t ld,
                         uint32_t flags);
+
+/* Rolled windows of staged rows (extract_features(roll_time_series(df, column_kind=...)), dataframe_functions.py:
+ * 376-603), between the two calls above:
+ *   tsfx_roll_staged      turns the staged series into staged windows, with the window arithmetic of tsfx_roll_windows:
+ *                         every kind rolls on its own, the shifts anchored to the longest (kind, id) series of the call.
+ *                         max_timeshift 0 means None (the longest series).  A window is a view on the staged values, so
+ *                         each kind keeps its row alignment.  A window is named (id, sort key of its naming row: last
+ *                         row for a positive direction, first for a negative one), or (id, row number of that row in
+ *                         its series) when the rows were staged without sort keys; the staged rows are the union of
+ *                         the names over all kinds, ascending.  Needs TSFX_FLAG_KEEP_SORT_KEYS on the stage call when
+ *                         sort keys were given.  Synchronises the stream once and returns the number of union windows
+ *                         in *n_rows_out and the longest window of every kind in max_len_per_kind (host, n_kinds
+ *                         entries; the exact longest window, which tsfx_extract_staged checks against each plan's
+ *                         limit).  TSFX_E_INVALID when two windows of one kind have the same name (sort keys tied at
+ *                         their naming rows; the reference would merge them into one series).  No feature kernel runs.
+ *                         No flags are defined for it yet: pass 0.
+ *   tsfx_staged_row_keys  copies the naming sort keys (raw int64 / float64 bits as staged, float64 -0.0 as +0.0; row
+ *                         numbers as int64 without sort keys) of the n_rows_out staged windows to out_keys (device, 8
+ *                         bytes each), asynchronously.  Valid until the next stage call.
+ * tsfx_extract_staged then extracts the windows: out_ids receives the id of every union window. */
+int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
+                     int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags);
+int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys);
 
 /* Page-locked host memory from the context's pool (freed blocks are cached: page-locking is slow). */
 void* tsfx_host_alloc(tsfx_ctx* ctx, size_t bytes);

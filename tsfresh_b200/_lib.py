@@ -18,6 +18,7 @@ FLAG_NO_NAN_CHECK = 4
 FLAG_IMPUTE = 8
 FLAG_ALL_MEDIANS = 16
 FLAG_CHECK_DEVICE_INPUT = 32
+FLAG_KEEP_SORT_KEYS = 64
 STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy default stream for tsfx_ctx_set_stream
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
@@ -37,7 +38,8 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_extract_long", "tsfx_roll_windows", "tsfx_get_timings",
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
-           "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged"]
+           "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged",
+           "tsfx_roll_staged", "tsfx_staged_row_keys"]
 
 
 def load():
@@ -88,6 +90,8 @@ def load():
                                                 ctypes.POINTER(i64), u32]
         lib.tsfx_stage_long_stacked.argtypes = [vp, vp, vp, i32, vp, vp, i32, i32, vp, i64, ctypes.POINTER(i64), vp, vp, u32]
         lib.tsfx_extract_staged.argtypes = [vp, vp, vp, vp, i32, u32]
+        lib.tsfx_roll_staged.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i64), vp, u32]
+        lib.tsfx_staged_row_keys.argtypes = [vp, vp]
         _lib = lib
         return lib
 
@@ -205,18 +209,34 @@ class Context:
         return stats
 
     def stage_long_stacked(self, ids_ptr, sort_ptr, sort_is_f64, values_ptr, kind_ptr, kind_is_i64, n_kinds, times_ptr,
-                           n_rows):
+                           n_rows, keep_sort_keys=False):
         """tsfx_stage_long_stacked on device rows (pointers as ints, 0 for an absent column): returns (number of union
-        ids, rows of every kind, longest series of every kind).  Synchronises the context's stream once."""
+        ids, rows of every kind, longest series of every kind).  Synchronises the context's stream once.
+        keep_sort_keys: keep the sort keys for roll_staged."""
         n_ids = ctypes.c_int64(0)
         rows = np.zeros(n_kinds, dtype=np.int64)
         max_len = np.zeros(n_kinds, dtype=np.int32)
         rc = self.lib.tsfx_stage_long_stacked(self.h, ctypes.c_void_p(ids_ptr), ctypes.c_void_p(sort_ptr or None),
                                               int(sort_is_f64), ctypes.c_void_p(values_ptr), ctypes.c_void_p(kind_ptr or None),
                                               int(kind_is_i64), int(n_kinds), ctypes.c_void_p(times_ptr or None), int(n_rows),
-                                              ctypes.byref(n_ids), _ptr(rows), _ptr(max_len), FLAG_DEVICE_PTRS)
+                                              ctypes.byref(n_ids), _ptr(rows), _ptr(max_len),
+                                              FLAG_DEVICE_PTRS | (FLAG_KEEP_SORT_KEYS if keep_sort_keys else 0))
         self.check(rc, "tsfx_stage_long_stacked")
         return n_ids.value, rows, max_len
+
+    def roll_staged(self, rolling_direction, max_timeshift, min_timeshift, n_kinds):
+        """tsfx_roll_staged: the staged series become their rolled windows (max_timeshift 0: None).  Returns (number of
+        union windows, longest window of every kind).  Synchronises the context's stream once."""
+        n_rows = ctypes.c_int64(0)
+        max_len = np.zeros(n_kinds, dtype=np.int32)
+        rc = self.lib.tsfx_roll_staged(self.h, int(rolling_direction), int(max_timeshift), int(min_timeshift),
+                                       ctypes.byref(n_rows), _ptr(max_len), 0)
+        self.check(rc, "tsfx_roll_staged")
+        return n_rows.value, max_len
+
+    def staged_row_keys(self, keys_ptr):
+        """tsfx_staged_row_keys: the naming sort keys of the staged windows into device memory (8 bytes each)"""
+        self.check(self.lib.tsfx_staged_row_keys(self.h, ctypes.c_void_p(keys_ptr)), "tsfx_staged_row_keys")
 
     def extract_staged(self, device_plans, ids_ptr, out_ptr, ld, flags=0):
         """tsfx_extract_staged: device_plans[k] is kind k's DevicePlan (None for a kind without rows)"""

@@ -19,6 +19,7 @@
 #include "tsfx_common.cuh"
 #include "tsfx_kernels.h"
 #include "tsfx_csr.h"
+#include "tsfx_roll.cuh"
 #include "tsfx_impute.h"
 #include "tsfx_select.h"
 
@@ -1482,10 +1483,14 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
     S.n_kinds = n_kinds;
     S.n_union = 0;
     S.d_times = nullptr;
+    S.d_keys = nullptr;
+    S.has_keys = false;
+    S.rolled = false;
     if (n_rows > 0) {
         std::string msg;
         int rc = stacked_stage(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values, kind_codes,
-                               kind_code_is_i64, n_kinds, row_time_ns, n_rows, ctx->stream, &msg);
+                               kind_code_is_i64, n_kinds, row_time_ns, n_rows, (flags & TSFX_FLAG_KEEP_SORT_KEYS) != 0,
+                               ctx->stream, &msg);
         if (rc) return fail(ctx, rc, msg);
         CK(cudaStreamSynchronize(ctx->stream));
         const StackedInfo& I = *S.h_info;
@@ -1562,6 +1567,59 @@ extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans,
     CK(cudaMemcpyAsync(out_ids, S.d_uid, (size_t)U * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->launches = launched;
     if (flags & TSFX_FLAG_IMPUTE) return impute_after_extract(ctx, out, U, total);
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
+                                int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags) {
+    (void)flags;
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (!S.valid || S.rolled) return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: no unrolled rows staged (tsfx_stage_long_stacked)");
+    if (!n_rows_out || !max_len_per_kind || rolling_direction == 0 || max_timeshift < 0 || min_timeshift < 0)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: bad arguments");
+    if (S.has_keys && !S.d_keys)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: the rows were staged without TSFX_FLAG_KEEP_SORT_KEYS");
+    S.valid = false;
+    *n_rows_out = 0;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
+    if (S.n_union == 0) { S.rolled = true; S.valid = true; return TSFX_OK; }
+    CK(cudaSetDevice(ctx->device));
+    const StackedInfo& I = *S.h_info;
+    // the shifts are anchored to the longest (kind, id) series; a window never has more rows than its series, and a
+    // series of L rows has at most one window per shift <= L
+    int32_t Lmax = 0;
+    int64_t rows = 0;
+    for (int k = 0; k < S.n_kinds; ++k) { Lmax = std::max(Lmax, I.kind_max_len[k]); rows += I.kind_rows[k]; }
+    if (max_timeshift == 0) max_timeshift = Lmax;
+    const RollSpec R = roll_spec(rolling_direction, max_timeshift, min_timeshift, Lmax);
+    const int64_t shifts = (Lmax - R.first) / R.amount + 1;
+    const int64_t series = I.kind_series[S.n_kinds];
+    const int64_t bound = std::min(rows, series > rows / shifts ? rows : series * shifts);
+    std::string msg;
+    int rc = stacked_roll(S, ctx->csr, rolling_direction, max_timeshift, min_timeshift, Lmax, bound, ctx->stream, &msg);
+    if (rc) return fail(ctx, rc, msg);
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (I.dup_names)
+        return fail(ctx, TSFX_E_INVALID, "two windows of one kind have the same name (id, sort key): the sort keys tie at "
+                                         "the rows that name them");
+    S.n_union = I.n_union;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = I.kind_max_len[k];
+    *n_rows_out = S.n_union;
+    S.valid = true;
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys) {
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    if (!S.rolled) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: no windows staged (tsfx_roll_staged)");
+    if (S.n_union == 0) return TSFX_OK;
+    if (!out_keys) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: NULL out_keys");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(out_keys, S.d_ukey, (size_t)S.n_union * 8, cudaMemcpyDeviceToDevice, ctx->stream));
     return TSFX_OK;
 }
 
@@ -1682,35 +1740,22 @@ extern "C" int64_t tsfx_roll_windows(const int64_t* begin, const int32_t* len, i
                                      int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                                      int64_t* win_begin, int32_t* win_len, int64_t* win_parent,
                                      int32_t* win_end_index, int64_t capacity) {
-    // dataframe_functions.py:340-373, 548-562.  rolling_direction > 0: the shifts are
-    // reversed(range(Lmax, 0, -rolling_direction)) where Lmax is the LONGEST series of the frame (:555-560), so
-    // window ends are anchored to Lmax for every series; shift t applies to a series of length L when t <= L,
-    // the window is rows [max(t-max_timeshift-1, 0), t), kept when it has at least min_timeshift+1 rows, and
-    // its id is (parent id, time of row t-1).
-    // rolling_direction < 0 (:351-356, 365-366): shifts range(1, Lmax+1, |rolling_direction|), the window is rows
-    // [t-1, min(t+max_timeshift, L)), same minimum length, id = (parent id, time of row t-1) -- the window's FIRST row.
-    // win_end_index is therefore "the row whose sort value names the window": last row (positive) / first row (negative).
+    // the window arithmetic (dataframe_functions.py:340-373, 548-562) is tsfx_roll.cuh's, shared with tsfx_roll_staged;
+    // win_end_index is "the row whose sort value names the window": last row (positive) / first row (negative).
     if (!begin || !len || n_series < 0 || rolling_direction == 0 || max_timeshift < 0 || min_timeshift < 0)
         return TSFX_E_INVALID;
     int32_t Lmax = 0;
     for (int64_t s = 0; s < n_series; ++s) { if (len[s] < 1) return TSFX_E_INVALID; Lmax = std::max(Lmax, len[s]); }
-    const int32_t amount = rolling_direction > 0 ? rolling_direction : -rolling_direction;
-    const int32_t first = rolling_direction > 0 ? (Lmax > 0 ? Lmax - ((Lmax - 1) / amount) * amount : 1) : 1;   // smallest shift
+    const RollSpec R = roll_spec(rolling_direction, max_timeshift, min_timeshift, Lmax);
     int64_t k = 0;
     for (int64_t s = 0; s < n_series; ++s) {
         const int32_t L = len[s];
-        for (int32_t t = first; t <= L; t += amount) {
-            int32_t lo, wl;
-            if (rolling_direction > 0) {
-                lo = t - max_timeshift - 1;
-                if (lo < 0) lo = 0;
-                wl = t - lo;
-            } else {
-                lo = t - 1;
-                const int64_t hi = std::min<int64_t>((int64_t)lo + max_timeshift + 1, L);
-                wl = (int32_t)(hi - lo);
-            }
-            if (wl < min_timeshift + 1) continue;
+        int32_t t0;
+        const int64_t n = roll_kept(R, L, &t0);
+        for (int64_t j = 0; j < n; ++j) {
+            const int32_t t = (int32_t)(t0 + j * R.amount);
+            int32_t lo;
+            const int32_t wl = roll_window(R, L, t, &lo);
             if (win_begin) {
                 if (k >= capacity) return TSFX_E_INVALID;
                 win_begin[k] = begin[s] + lo;

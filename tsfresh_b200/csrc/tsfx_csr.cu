@@ -3,9 +3,11 @@
 #include <thrust/iterator/counting_iterator.h>
 #include <thrust/iterator/transform_iterator.h>
 #include <algorithm>
+#include <cstddef>
 
 #include "../../include/tsfx.h"
 #include "tsfx_csr.h"
+#include "tsfx_roll.cuh"
 
 namespace tsfx {
 
@@ -228,18 +230,16 @@ void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, c
     k_check_views<<<grid_for(n_series * 32, 256), 256, 0, st>>>(d_values, n_values, d_begin, d_len, n_series, W.d_info);
 }
 
-int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, const float* d_values,
-                  int64_t n, int64_t min_block, int max_blocks, bool check_nan, cudaStream_t st, std::string* msg) {
+// Stable sort of the row index by (id, sort key) (sort key nullptr: by id alone): *perm_out = input row of every sorted
+// row, and S_KEY_B holds the sorted ids as ordered keys (key_i64).
+static int sort_rows(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, int64_t n, cudaStream_t st,
+                     std::string* msg, uint32_t** perm_out_) {
     const int threads = 256;
     const int blocks = grid_for(n, threads);
-    CKE(W.init_info(), "alloc info");
-    CKE(cudaMemsetAsync(W.d_info, 0, sizeof(CsrInfo), st), "memset info");
-    if (check_nan) csr_check_nan(W, d_values, n, st);
     CKE(W.reserve(S_PERM_A, n * 4), "alloc perm");
     CKE(W.reserve(S_PERM_B, n * 4), "alloc perm");
     CKE(W.reserve(S_KEY_A, n * 8), "alloc key");
     CKE(W.reserve(S_KEY_B, n * 8), "alloc key");
-    CKE(W.reserve(S_IDS_SORTED, n * 8), "alloc ids sorted");
     uint32_t *pa = (uint32_t*)W.bufs[S_PERM_A], *pb = (uint32_t*)W.bufs[S_PERM_B];
     uint64_t *ka = (uint64_t*)W.bufs[S_KEY_A], *kb = (uint64_t*)W.bufs[S_KEY_B];
     size_t tb = 0;
@@ -255,6 +255,21 @@ int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys,
     k_gather_id_keys<<<blocks, threads, 0, st>>>(d_ids, perm, n, ka);
     uint32_t* perm_out = (perm == pa) ? pb : pa;
     CKE(cub::DeviceRadixSort::SortPairs(W.bufs[S_TEMP], tb, ka, kb, perm, perm_out, (int)n, 0, 64, st), "radix sort B");
+    *perm_out_ = perm_out;
+    return TSFX_OK;
+}
+
+int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, const float* d_values,
+                  int64_t n, int64_t min_block, int max_blocks, bool check_nan, cudaStream_t st, std::string* msg) {
+    const int threads = 256;
+    const int blocks = grid_for(n, threads);
+    CKE(W.init_info(), "alloc info");
+    CKE(cudaMemsetAsync(W.d_info, 0, sizeof(CsrInfo), st), "memset info");
+    if (check_nan) csr_check_nan(W, d_values, n, st);
+    uint32_t* perm_out = nullptr;
+    if (int rc = sort_rows(W, d_ids, d_keys, is_f64, n, st, msg, &perm_out)) return rc;
+    CKE(W.reserve(S_IDS_SORTED, n * 8), "alloc ids sorted");
+    uint64_t *ka = (uint64_t*)W.bufs[S_KEY_A], *kb = (uint64_t*)W.bufs[S_KEY_B];
     // gather: sorted ids, sorted values (into pass-A key storage, free by now)
     k_gather_final<<<blocks, threads, 0, st>>>(kb, d_values, perm_out, n, (int64_t*)W.bufs[S_IDS_SORTED], (float*)ka);
     W.d_values = (float*)ka;
@@ -267,7 +282,11 @@ int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys,
 
 // ---------------------------------------------------------------------------------------------------------------------
 // stacked long format (tsfx_csr.h)
-enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T_LEN, T_ROW, T_UID, T_INFO };
+enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T_LEN, T_ROW, T_UID, T_INFO, T_KEYS,
+       // stacked_roll: per-series window offsets, per-window begin / len / union row / parent id / name, scanned name
+       // flags, union windows' names
+       R_OFF, R_BEGIN, R_LEN, R_ROW, R_ID, R_KEY, R_SCAN, R_UID, R_UKEY, T_SLOTS };
+static_assert(T_SLOTS <= 24, "StackedWorkspace::bufs");
 
 cudaError_t StackedWorkspace::reserve(int slot, size_t bytes) {
     if (bytes <= caps[slot]) return cudaSuccess;
@@ -285,11 +304,12 @@ cudaError_t StackedWorkspace::keep_ids(const int64_t* d_src, int64_t n, cudaStre
     return cudaMemcpyAsync(d_uid, d_src, (size_t)n * 8, cudaMemcpyDeviceToDevice, st);
 }
 void StackedWorkspace::release() {
-    for (int i = 0; i < 12; ++i) { if (bufs[i]) cudaFree(bufs[i]); bufs[i] = nullptr; caps[i] = 0; }
+    for (int i = 0; i < T_SLOTS; ++i) { if (bufs[i]) cudaFree(bufs[i]); bufs[i] = nullptr; caps[i] = 0; }
     if (h_info) cudaFreeHost(h_info);
     h_info = nullptr; d_info = nullptr;
     d_values = nullptr; d_times = nullptr; d_begin = nullptr; d_len = nullptr; d_row = nullptr; d_uid = nullptr;
-    valid = false;
+    d_keys = nullptr; d_ukey = nullptr;
+    valid = false; rolled = false;
 }
 
 #define STACK_TILE 4096          // rows per CTA of the counting sort
@@ -324,13 +344,15 @@ __global__ void __launch_bounds__(STACK_THREADS) k_stack_count(const uint32_t* _
 
 // Stable scatter of the counting sort: each tile walks its rows in order, 256 at a time; a row's destination is its
 // kind's running base in this tile + the rows of that kind in earlier warps of the step + its rank among its warp's
-// rows of the same kind (__match_any_sync).  Gathers the value (already in CSR order), the union row and the time.
+// rows of the same kind (__match_any_sync).  Gathers the value (already in CSR order), the union row, the time and the
+// sort key (the last two when asked for).
 __global__ void __launch_bounds__(STACK_THREADS) k_stack_scatter(const uint8_t* __restrict__ code, const int* __restrict__ offs,
                                                                  int n_kinds, int64_t n, const float* __restrict__ vals,
                                                                  const int32_t* __restrict__ urow, const int64_t* __restrict__ times,
+                                                                 const uint64_t* __restrict__ keys,
                                                                  const uint32_t* __restrict__ perm, const StackedInfo* info,
                                                                  float* __restrict__ out_vals, int32_t* __restrict__ out_row,
-                                                                 int64_t* __restrict__ out_times) {
+                                                                 int64_t* __restrict__ out_times, uint64_t* __restrict__ out_keys) {
     constexpr int W = STACK_THREADS / 32;
     __shared__ int64_t base[TSFX_MAX_KINDS];
     __shared__ int cnt[W][TSFX_MAX_KINDS];
@@ -353,6 +375,7 @@ __global__ void __launch_bounds__(STACK_THREADS) k_stack_scatter(const uint8_t* 
             out_vals[dst] = vals[i];
             out_row[dst] = urow[i];
             if (times) out_times[dst] = times[perm[i]];
+            if (keys) out_keys[dst] = keys[perm[i]];
         }
         __syncthreads();
         for (int kk = threadIdx.x; kk < n_kinds; kk += blockDim.x) {
@@ -442,9 +465,12 @@ __global__ void k_stack_finish(const CsrInfo* csr, StackedInfo* info) {
 
 int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
                   const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
-                  int64_t n, cudaStream_t st, std::string* msg) {
+                  int64_t n, bool keep_keys, cudaStream_t st, std::string* msg) {
     S.valid = false;
+    S.rolled = false;
     S.n_kinds = n_kinds;
+    S.has_keys = d_keys != nullptr;
+    S.keys_f64 = d_keys && keys_f64;
     if (!S.h_info) CKE(cudaHostAlloc((void**)&S.h_info, sizeof(StackedInfo), cudaHostAllocDefault), "alloc info");
     CKE(S.reserve(T_INFO, sizeof(StackedInfo)), "alloc info");
     S.d_info = (StackedInfo*)S.bufs[T_INFO];
@@ -464,12 +490,15 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     CKE(S.reserve(T_LEN, (size_t)n * 4), "alloc len");
     CKE(S.reserve(T_ROW, (size_t)n * 4), "alloc map");
     if (d_times) CKE(S.reserve(T_TIMES, (size_t)n_pad * 8), "alloc times");
+    keep_keys = keep_keys && d_keys;
+    if (keep_keys) CKE(S.reserve(T_KEYS, (size_t)n_pad * 8), "alloc keys");
     uint8_t* code = (uint8_t*)S.bufs[T_CODE];
     int32_t* urow = (int32_t*)S.bufs[T_UROW];      // union row of every CSR row; later the series index of every staged row
     int* counts = (int*)S.bufs[T_COUNTS];
     int32_t* srow = (int32_t*)S.bufs[T_SROW];
     S.d_values = (float*)S.bufs[T_VALS];
     S.d_times = d_times ? (int64_t*)S.bufs[T_TIMES] : nullptr;
+    S.d_keys = keep_keys ? (uint64_t*)S.bufs[T_KEYS] : nullptr;
     S.d_begin = (int64_t*)S.bufs[T_BEGIN];
     S.d_len = (int32_t*)S.bufs[T_LEN];
     S.d_row = (int32_t*)S.bufs[T_ROW];
@@ -491,14 +520,190 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     CKE(cudaMemsetAsync(counts + n_counts - 1, 0, 4, st), "memset counts");
     CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb2, counts, counts, (int)n_counts, st), "kind offsets");
     k_stack_kind_rows<<<1, 1, 0, st>>>(counts, n_kinds, n_tiles, S.d_info);
-    k_stack_scatter<<<n_tiles, STACK_THREADS, 0, st>>>(code, counts, n_kinds, n, W.d_values, urow, d_times, W.d_perm,
-                                                       S.d_info, S.d_values, srow, S.d_times);
+    k_stack_scatter<<<n_tiles, STACK_THREADS, 0, st>>>(code, counts, n_kinds, n, W.d_values, urow, d_times,
+                                                       keep_keys ? d_keys : nullptr, W.d_perm, S.d_info, S.d_values, srow,
+                                                       S.d_times, S.d_keys);
     CKE(cudaGetLastError(), "kind scatter kernel");
     CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb3, series_start, urow, (int)(n_pad + 1), st), "series index");
     k_stack_series<<<grid_for(n_pad, 256), 256, 0, st>>>(urow, start, n_pad, S.d_begin, S.d_row);
     k_stack_lengths<<<grid_for(n / 4 + 1, 256), 256, 0, st>>>(urow, n_pad, n_kinds, S.d_begin, S.d_len, S.d_info);
     k_stack_finish<<<1, 1, 0, st>>>(W.d_info, S.d_info);
     CKE(cudaGetLastError(), "series kernels");
+    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
+    return TSFX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// rolled windows of the staged series (stacked_roll)
+
+// kind whose series range holds series s (the last of kinds that start at the same series is the only one with series)
+__device__ __forceinline__ int kind_of_series(const StackedInfo* info, int n_kinds, int64_t s) {
+    int lo = 0, hi = n_kinds;
+    while (hi - lo > 1) { const int m = (lo + hi) >> 1; if (info->kind_series[m] <= s) lo = m; else hi = m; }
+    return lo;
+}
+
+// name of the window whose naming row is row r of the series at staged row b: the row's sort key (float64 -0.0 made
+// +0.0, which pandas holds equal to it), or r itself without sort keys
+__device__ __forceinline__ uint64_t window_name(const uint64_t* __restrict__ keys, int keys_f64, int64_t b, int32_t r) {
+    if (!keys) return (uint64_t)r;
+    const uint64_t k = keys[b + r];
+    return keys_f64 && k == 0x8000000000000000ull ? 0ull : k;
+}
+
+// windows of every series into cnt[s]; each kind's longest window into info->kind_max_len (zeroed by the caller).  The
+// window lengths are monotone in the shift, so a series' longest window is its first or its last.
+__global__ void k_roll_count(const int32_t* __restrict__ len, int64_t n_series, RollSpec R, int n_kinds,
+                             int32_t* __restrict__ cnt, StackedInfo* info) {
+    __shared__ int mx[TSFX_MAX_KINDS];
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) mx[k] = 0;
+    __syncthreads();
+    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; s < n_series; s += stride) {
+        const int32_t L = len[s];
+        int32_t t0, lo;
+        const int64_t n = roll_kept(R, L, &t0);
+        cnt[s] = (int32_t)n;
+        if (n > 0) {
+            const int32_t first = roll_window(R, L, t0, &lo);
+            const int32_t last = roll_window(R, L, (int32_t)(t0 + (n - 1) * R.amount), &lo);
+            atomicMax(&mx[kind_of_series(info, n_kinds, s)], max(first, last));
+        }
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
+}
+
+// One warp per series, one lane per window: the window's view on the staged values, its parent id and its name.  Two
+// windows of one series with the same name (sort keys tied at their naming rows) set info->dup_names.  The slots
+// [off[n_series], bound) get the name that sorts after every real one (id INT64_MAX, key 0x7fff...f: the largest
+// int64, or a NaN above every float64 key).
+__global__ void k_roll_fill(const int64_t* __restrict__ begin, const int32_t* __restrict__ len, const int32_t* __restrict__ row,
+                            const int64_t* __restrict__ uid, const uint64_t* __restrict__ keys, int keys_f64,
+                            const int32_t* __restrict__ off, int64_t n_series, int64_t bound, RollSpec R,
+                            int64_t* __restrict__ wbegin, int32_t* __restrict__ wlen, int64_t* __restrict__ wid,
+                            uint64_t* __restrict__ wkey, StackedInfo* info) {
+    const int lane = threadIdx.x & 31;
+    int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    int dup = 0;
+    for (; s < n_series; s += n_warps) {                  // warp-uniform
+        const int64_t b = begin[s];
+        const int32_t L = len[s];
+        const int64_t id = uid[row[s]];
+        const int32_t o = off[s], n = off[s + 1] - o;
+        int32_t t0;
+        roll_kept(R, L, &t0);
+        for (int32_t j = lane; j < n; j += 32) {
+            const int32_t t = (int32_t)(t0 + (int64_t)j * R.amount);
+            int32_t lo;
+            const int32_t wl = roll_window(R, L, t, &lo);
+            const uint64_t name = window_name(keys, keys_f64, b, t - 1);
+            wbegin[o + j] = b + lo;
+            wlen[o + j] = wl;
+            wid[o + j] = id;
+            wkey[o + j] = name;
+            if (j > 0 && keys) dup |= name == window_name(keys, keys_f64, b, t - R.amount - 1);
+        }
+    }
+    if (__any_sync(0xffffffffu, dup) && lane == 0) atomicOr(&info->dup_names, 1);
+    int64_t i = off[n_series] + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (const int64_t stride = (int64_t)gridDim.x * blockDim.x; i < bound; i += stride) {
+        wid[i] = INT64_MAX;
+        wkey[i] = 0x7fffffffffffffffull;
+    }
+}
+
+// 1 where sorted window i starts a new name (window 0 excluded, the sentinel slots from *n_windows on are 0): the
+// inclusive scan is the union row of every sorted window
+struct NameChange {
+    const int64_t* wid;
+    const uint64_t* wkey;
+    const uint32_t* perm;
+    const int32_t* n_windows;
+    __device__ int operator()(int64_t i) const {
+        if (i == 0 || i >= *n_windows) return 0;
+        const uint32_t a = perm[i - 1], b = perm[i];
+        return wid[a] != wid[b] || wkey[a] != wkey[b];
+    }
+};
+
+// union row of every window, name of every union row, the union size
+__global__ void k_roll_union(const uint32_t* __restrict__ perm, const int32_t* __restrict__ scan, const int32_t* __restrict__ n_windows,
+                             const int64_t* __restrict__ wid, const uint64_t* __restrict__ wkey, int32_t* __restrict__ wrow,
+                             int64_t* __restrict__ uid, uint64_t* __restrict__ ukey, StackedInfo* info) {
+    const int64_t nw = *n_windows;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    if (i == 0) info->n_union = nw > 0 ? (int64_t)scan[nw - 1] + 1 : 0;
+    for (; i < nw; i += stride) {
+        const uint32_t w = perm[i];
+        const int32_t u = scan[i];
+        wrow[w] = u;
+        if (i == 0 || u != scan[i - 1]) { uid[u] = wid[w]; ukey[u] = wkey[w]; }
+    }
+}
+
+// each kind's series range becomes its window range
+__global__ void k_roll_kinds(const int32_t* __restrict__ off, int n_kinds, StackedInfo* info) {
+    for (int k = threadIdx.x; k <= n_kinds; k += blockDim.x) info->kind_series[k] = off[info->kind_series[k]];
+}
+
+int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
+                 int32_t Lmax, int64_t bound, cudaStream_t st, std::string* msg) {
+    const int n_kinds = S.n_kinds;
+    const int64_t ns = S.h_info->kind_series[n_kinds];
+    const RollSpec R = roll_spec(rolling_direction, max_timeshift, min_timeshift, Lmax);
+    const size_t nb = (size_t)std::max<int64_t>(bound, 1);
+    CKE(S.reserve(R_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
+    CKE(S.reserve(R_BEGIN, nb * 8), "alloc windows");
+    CKE(S.reserve(R_LEN, nb * 4), "alloc windows");
+    CKE(S.reserve(R_ROW, nb * 4), "alloc windows");
+    CKE(S.reserve(R_ID, nb * 8), "alloc windows");
+    CKE(S.reserve(R_KEY, nb * 8), "alloc windows");
+    CKE(S.reserve(R_SCAN, nb * 4), "alloc windows");
+    CKE(S.reserve(R_UID, nb * 8), "alloc windows");
+    CKE(S.reserve(R_UKEY, nb * 8), "alloc windows");
+    int32_t* off = (int32_t*)S.bufs[R_OFF];
+    int64_t* wbegin = (int64_t*)S.bufs[R_BEGIN];
+    int32_t* wlen = (int32_t*)S.bufs[R_LEN];
+    int32_t* wrow = (int32_t*)S.bufs[R_ROW];
+    int64_t* wid = (int64_t*)S.bufs[R_ID];
+    uint64_t* wkey = (uint64_t*)S.bufs[R_KEY];
+    int32_t* scan = (int32_t*)S.bufs[R_SCAN];
+    const int keys_f64 = S.d_keys && S.keys_f64;
+    uint32_t* perm = nullptr;
+    size_t tb1 = 0, tb2 = 0;
+    NameChange change{wid, wkey, nullptr, off + ns};
+    thrust::counting_iterator<int64_t> rows(0);
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb1, off, off, (int)(ns + 1), st), "scan size");
+    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st), "scan size");
+    CKE(S.reserve(T_TEMP, std::max(tb1, tb2)), "alloc temp");
+    // windows per series, their offsets, each kind's longest window
+    CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
+        "memset info");
+    CKE(cudaMemsetAsync(off + ns, 0, 4, st), "memset offsets");
+    k_roll_count<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, R, n_kinds, off, S.d_info);
+    CKE(cudaGetLastError(), "window count kernel");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb1, off, off, (int)(ns + 1), st), "window offsets");
+    k_roll_fill<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(
+        S.d_begin, S.d_len, S.d_row, S.d_uid, S.d_keys, keys_f64, off, ns, bound, R, wbegin, wlen, wid, wkey, S.d_info);
+    CKE(cudaGetLastError(), "window fill kernel");
+    // the union of the names: sort (id, name), flag and scan the distinct pairs
+    if (int rc = sort_rows(W, wid, wkey, keys_f64, bound, st, msg, &perm)) return rc;
+    change.perm = perm;
+    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st),
+        "union rows");
+    S.d_uid = (int64_t*)S.bufs[R_UID];
+    S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
+    k_roll_union<<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, wid, wkey, wrow, S.d_uid, S.d_ukey, S.d_info);
+    k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
+    CKE(cudaGetLastError(), "union kernels");
+    S.d_begin = wbegin;
+    S.d_len = wlen;
+    S.d_row = wrow;
+    S.rolled = true;
     CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
     return TSFX_OK;
 }

@@ -94,7 +94,7 @@ struct StackedInfo {              // written by the device, read once by the hos
     int32_t bad_kind;             // a kind code outside 0 .. n_kinds-1
     int32_t nan_values;
     int32_t nan_keys;             // a float64 sort key is NaN
-    int32_t pad;
+    int32_t dup_names;            // stacked_roll: two windows of one kind have the same name
     int64_t n_union;              // distinct ids over all kinds
     int64_t kind_row[TSFX_MAX_KINDS + 1];      // kind k's rows are [kind_row[k], + kind_rows[k]) of the partitioned arrays
     int64_t kind_rows[TSFX_MAX_KINDS];
@@ -109,14 +109,19 @@ struct StackedWorkspace {
     int64_t* d_begin = nullptr;   // series s = d_values[d_begin[s] .. + d_len[s])
     int32_t* d_len = nullptr;
     int32_t* d_row = nullptr;     // union row of series s
-    int64_t* d_uid = nullptr;     // union ids, ascending (keep_ids)
+    int64_t* d_uid = nullptr;     // union ids, ascending (keep_ids); after stacked_roll the parent id of every window
+    uint64_t* d_keys = nullptr;   // sort keys (raw bits) in the order of d_values (stacked_stage with keep_keys)
+    uint64_t* d_ukey = nullptr;   // after stacked_roll: naming sort key of every union window (raw bits)
     StackedInfo* h_info = nullptr;   // pinned
     StackedInfo* d_info = nullptr;
     int n_kinds = 0;
     int64_t n_union = 0;
     bool valid = false;           // staged and not yet consumed
-    void* bufs[12] = {nullptr};
-    size_t caps[12] = {0};
+    bool has_keys = false;        // the rows came with sort keys
+    bool keys_f64 = false;        //   float64 ones
+    bool rolled = false;          // the staged series have been turned into windows (stacked_roll)
+    void* bufs[24] = {nullptr};
+    size_t caps[24] = {0};
     cudaError_t reserve(int slot, size_t bytes);
     cudaError_t keep_ids(const int64_t* d_src, int64_t n, cudaStream_t st);   // d_uid = a copy of n union ids
     void release();
@@ -124,10 +129,21 @@ struct StackedWorkspace {
 
 // Stages n_rows device rows (ids, sort keys (nullptr: input order), float32 values, kind codes (int32 / int64; nullptr:
 // every row is kind 0), optional int64 row times) into S, then copies S.d_info to S.h_info.  Asynchronous: the caller
-// synchronises and checks the flags before it relies on the sizes.  Uses W's sort buffers as scratch.
+// synchronises and checks the flags before it relies on the sizes.  Uses W's sort buffers as scratch.  keep_keys: the
+// sort keys follow the rows into S.d_keys (stacked_roll names its windows by them).
 int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
                   const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
-                  int64_t n_rows, cudaStream_t st, std::string* msg);
+                  int64_t n_rows, bool keep_keys, cudaStream_t st, std::string* msg);
+
+// Rolled windows (roll_time_series, tsfx_roll.cuh) of the staged series, as new staged series: every window is a view
+// (d_begin, d_len) on the unchanged d_values, so each kind keeps its aligned rows.  Per series a count of its windows, a
+// scan, then a fill of one warp per series; the windows' names (parent id, sort key of the naming row, or its row number
+// without sort keys) are sorted with W's radix passes, and the distinct names, flagged and scanned, are the union rows:
+// d_row of every window, d_uid / d_ukey of every union row.  d_info gets the window ranges of the kinds (kind_series),
+// their longest windows (kind_max_len), n_union and dup_names, and is copied to h_info (the caller synchronises).
+// Lmax = the longest staged series (the shifts' anchor); bound >= the number of windows.
+int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
+                 int32_t Lmax, int64_t bound, cudaStream_t st, std::string* msg);
 
 // out[r * ld + c] = NaN for r < n_rows, c < n_cols
 cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cudaStream_t st);

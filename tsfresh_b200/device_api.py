@@ -15,6 +15,13 @@ takes one tensor per column of a long frame, rows in any order, and returns what
 with column_kind: one row per id of any kind (ids ascending), one column block per kind.  Its row count is only known
 after the rows are grouped, so the library stages the rows first (tsfx_stage_long_stacked, one host synchronisation)
 and torch then allocates the result that the extraction (tsfx_extract_staged) fills.
+
+    X, window_ids, window_keys, columns = extract_features_rolled_device(ids, values, sort, kind, kinds=[...],
+                                                                         rolling_direction=32, max_timeshift=255)
+
+is extract_features(roll_time_series(frame, ...)) for the same rows: between the two calls, tsfx_roll_staged turns the
+staged series into their rolled windows (views on the staged values) and their union of names, with a second host
+synchronisation to learn the number of windows.
 """
 import numpy as np
 import pandas as pd
@@ -227,8 +234,62 @@ def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=Non
     columns.  Runs on torch's current stream and blocks the host once, to learn the number of ids.  Raises ValueError for
     NaN values or sort keys, kind codes out of range and series longer than their kind's plan allows, before any feature
     kernel runs."""
+    X, row_ids, _, columns = _extract_staged(ids, values, sort, kind, kinds, times, None, default_fc_parameters,
+                                             kind_to_fc_parameters, impute_function)
+    return X, row_ids, columns
+
+
+_I32_MAX = (1 << 31) - 1
+
+
+def _roll_args(rolling_direction, max_timeshift, min_timeshift):
+    """roll_time_series's argument errors, with its messages; then the arguments as tsfx_roll_staged takes them (int32,
+    max_timeshift 0 for None; values beyond int32 act as the largest one would)"""
+    if rolling_direction == 0:
+        raise ValueError("Rolling direction of 0 is not possible")
+    if max_timeshift is not None and max_timeshift <= 0:
+        raise ValueError("max_timeshift needs to be positive!")
+    if min_timeshift < 0:
+        raise ValueError("min_timeshift needs to be positive or zero!")
+    direction = max(-_I32_MAX, min(int(rolling_direction), _I32_MAX))
+    return direction, 0 if max_timeshift is None else min(int(max_timeshift), _I32_MAX), min(int(min_timeshift), _I32_MAX)
+
+
+def extract_features_rolled_device(ids, values, sort=None, kind=None, *, kinds=None, rolling_direction=1, max_timeshift=None,
+                                   min_timeshift=0, default_fc_parameters=None, kind_to_fc_parameters=None,
+                                   impute_function=None):
+    """Extracts features from the rolled windows of long-format rows held in CUDA tensors into a CUDA tensor.
+
+    ids, values, sort, kind, kinds, default_fc_parameters, kind_to_fc_parameters and impute_function: as
+    extract_features_long_device.  rolling_direction, max_timeshift and min_timeshift: as roll_time_series.
+
+    Returns (X, window_ids, window_keys, columns), what extract_features returns for roll_time_series(df, column_id="id",
+    column_sort="time", column_kind="kind", ...) of the equivalent frame: row r of X is the window named (window_ids[r],
+    window_keys[r]), names ascending.  window_ids is int64; window_keys has the sort keys' dtype, or is int64 holding the
+    row number inside the series with sort=None.  A window is named by its last row for a positive direction and by its
+    first row for a negative one.  Every kind rolls on its own, the shifts anchored to the longest (kind, id) series; the
+    rows are the union of the window names over all kinds, NaN where a kind has no window of that name.  Like the rolled
+    frame, linear_trend_timewise is skipped.  The quadratic entropies' length limit applies to each window, not to the
+    series it comes from.
+
+    Runs on torch's current stream and blocks the host twice: to group the rows and to count the windows.  Raises
+    roll_time_series's errors for its arguments before the device is touched, and ValueError for two windows of one kind
+    with the same name (sort keys tied at their naming rows), NaN values or sort keys, kind codes out of range and windows
+    longer than their kind's plan allows, before any feature kernel runs."""
+    roll = _roll_args(rolling_direction, max_timeshift, min_timeshift)
+    return _extract_staged(ids, values, sort, kind, kinds, None, roll, default_fc_parameters, kind_to_fc_parameters,
+                           impute_function)
+
+
+def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_parameters, kind_to_fc_parameters,
+                    impute_function):
+    """(X, row ids, row keys, columns) of long-format rows, staged by kind and extracted; with roll = (direction,
+    max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows' naming keys,
+    else None)."""
     import torch
     n, kinds = _long_layout(ids, values, sort, kind, kinds, times)
+    if roll is not None and n <= 1:
+        raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
     default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
     plans = [_kind_plan(k, default_fc_parameters, kind_to_fc_parameters, has_datetime_index=times is not None)
              for k in kinds]
@@ -239,6 +300,7 @@ def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=Non
         if t is not None and t.device != dev:
             raise ValueError("%s is on %s, values on %s" % (name, t.device, dev))
     mode = _lib.IMPUTE_RANGE if impute_function is impute else _lib.IMPUTE_ZERO if impute_function is impute_dataframe_zero else None
+    row_keys = None
     with torch.cuda.device(dev):
         v = values.contiguous() if values.dtype == torch.float32 else values.to(torch.float32).contiguous()
         i = ids.contiguous()
@@ -250,24 +312,28 @@ def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=Non
         with ctx.lock:
             ctx.set_stream(stream or _lib.STREAM_LEGACY)
             try:
-                n_ids, rows, _ = ctx.stage_long_stacked(
+                n_rows, rows, _ = ctx.stage_long_stacked(
                     i.data_ptr(), 0 if s is None else s.data_ptr(), s is not None and s.dtype == torch.float64,
                     v.data_ptr(), 0 if k is None else k.data_ptr(), k is not None and k.dtype == torch.int64, len(kinds),
-                    0 if t is None else t.data_ptr(), n)
+                    0 if t is None else t.data_ptr(), n, keep_sort_keys=roll is not None)
+                if roll is not None:
+                    n_rows, _ = ctx.roll_staged(*roll, len(kinds))
+                    row_keys = torch.empty(n_rows, dtype=torch.int64 if s is None else s.dtype, device=dev)
+                    ctx.staged_row_keys(row_keys.data_ptr())
                 present = [c for c in range(len(kinds)) if rows[c] > 0]
                 columns = [name for c in present for name in plans[c][1]]
                 width = len(columns)
-                X = torch.empty((n_ids, width), dtype=torch.float64, device=dev)
-                row_ids = torch.empty(n_ids, dtype=torch.int64, device=dev)
+                X = torch.empty((n_rows, width), dtype=torch.float64, device=dev)
+                row_ids = torch.empty(n_rows, dtype=torch.int64, device=dev)
                 dps = [_device_plan(ctx, plans[c][0]) if rows[c] > 0 else None for c in range(len(kinds))]
                 ctx.extract_staged(dps, row_ids.data_ptr(), X.data_ptr(), width,
                                    _lib.FLAG_IMPUTE if mode == _lib.IMPUTE_RANGE else 0)
-                if mode == _lib.IMPUTE_ZERO and n_ids and width:
-                    ctx.impute_device(X.data_ptr(), n_ids, width, mode)
+                if mode == _lib.IMPUTE_ZERO and n_rows and width:
+                    ctx.impute_device(X.data_ptr(), n_rows, width, mode)
             finally:
                 ctx.set_stream(None)
     if impute_function is not None and mode is None:
         df = pd.DataFrame(X.cpu().numpy(), columns=columns)
         impute_function(df)
         X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
-    return X, row_ids, columns
+    return X, row_ids, row_keys, columns
