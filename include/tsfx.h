@@ -34,7 +34,7 @@
 extern "C" {
 #endif
 
-#define TSFX_VERSION 3
+#define TSFX_VERSION 4
 
 /* error codes */
 #define TSFX_OK 0
@@ -241,9 +241,9 @@ int tsfx_extract_dense(tsfx_ctx* ctx, const tsfx_plan* plan, const float* values
  * Rows that already arrive ordered by (id, sort key) take the pipelined path: one pass over the id column, one host
  * synchronisation for the sizes, then the sort-key / value columns are copied in row blocks while the kernels of the
  * previous blocks run and their result rows travel back.  Any other order is sorted on the device first.
- * Host pointers may be pageable (staged through pinned memory by worker threads) or page-locked.  With
- * TSFX_FLAG_DEVICE_PTRS every pointer (ids, sort_keys, values, out_ids, out) is a device pointer; the call still
- * synchronises once to learn the sizes. */
+ * Host pointers may be pageable (staged through pinned memory by worker threads) or page-locked; TSFX_FLAG_DEVICE_PTRS
+ * is TSFX_E_INVALID.  Rows already on the device go through tsfx_stage_long_stacked + tsfx_extract_staged: with
+ * kind_codes NULL and n_kinds 1 they give the same ids and matrix. */
 int tsfx_extract_long(tsfx_ctx* ctx, const tsfx_plan* plan, const int64_t* ids, const void* sort_keys,
                       int32_t sort_key_is_f64, const float* values, int64_t n_rows, int64_t* out_ids,
                       double* out, int64_t out_capacity, int64_t* n_series_out, uint32_t flags);

@@ -1,6 +1,6 @@
 """Stage (a) of the hot path through the C ABI (tsfx_extract_long_alloc / tsfx_extract_long / tsfx_extract_long_kinds):
 the pipelined path for rows ordered by (id, sort key), the device sort for every other order, the NaN scan, pinned
-and pageable host buffers, device pointers.  Restates the reference's adapter behaviour
+and pageable host buffers; device rows go through the staged calls.  Restates the reference's adapter behaviour
 (tsfresh/feature_extraction/data.py:217-230, 280-291; row-order invariance: test_extraction.py:207-237)."""
 import numpy as np
 import pytest
@@ -30,12 +30,13 @@ def frame(n_series, rng, min_len=3, max_len=12):
     return ids, t, v, lens
 
 
-def dense_reference(dp, ids, t, v):
-    """the same rows through the CSR entry point after a host-side lexsort"""
+def dense_reference(dp, ids, t, v, times=None, flags=0):
+    """the same rows (and row times) through the CSR entry point after a host-side lexsort"""
     order = np.lexsort((t, ids))
     ids_s, v_s = ids[order], v[order]
     uid, start, cnt = np.unique(ids_s, return_index=True, return_counts=True)
-    return uid, dp.extract_csr(v_s, start.astype(np.int64), cnt.astype(np.int32))
+    return uid, dp.extract_csr(v_s, start.astype(np.int64), cnt.astype(np.int32), flags=flags,
+                               times=None if times is None else times[order])
 
 
 def test_ordered_rows_take_the_pipelined_path_in_several_blocks(env):
@@ -70,6 +71,35 @@ def test_any_row_order_gives_the_same_matrix(env):
     assert np.array_equal(mat, ref, equal_nan=True)
     uid, mat = dp.extract_long(ids, None, v)
     assert np.array_equal(mat, ref, equal_nan=True)
+    orders = {"ordered": np.arange(len(ids)), "shuffled": perm, "keys out of order": order}
+    # linear_trend_timewise: the row times follow the rows through the sort, also when it runs after the streamed pass
+    from tsfresh_b200 import _lib
+    from tsfresh_b200._lib import DevicePlan
+    tw = DevicePlan(ctx, Plan({"mean": None, "linear_trend_timewise": [{"attr": a} for a in ("slope", "intercept", "stderr")]},
+                              has_datetime_index=True))
+    times = (t * 3600 + rng.integers(0, 1800, len(t))) * 1_000_000_000              # hours apart, jittered
+    uid_tw, ref_tw = dense_reference(tw, ids, t, v, times=times)
+    for name, o in orders.items():
+        uid, mat = tw.extract_long(ids[o], t[o], v[o], times=times[o])
+        assert np.array_equal(uid, uid_tw) and np.array_equal(mat, ref_tw, equal_nan=True), name
+    tw.close()
+    # TSFX_FLAG_IMPUTE on a matrix with non-finite features (infinite values)
+    vi = v.copy()
+    vi[rng.choice(len(v), 40, replace=False)] = np.inf
+    _, raw = dense_reference(dp, ids, t, vi)
+    _, ref_imp = dense_reference(dp, ids, t, vi, flags=_lib.FLAG_IMPUTE)
+    assert not np.isfinite(raw).all() and np.isfinite(ref_imp).all()
+    for name, o in orders.items():
+        uid, mat = dp.extract_long(ids[o], t[o], vi[o], flags=_lib.FLAG_IMPUTE)
+        assert np.array_equal(uid, uid_ref) and np.array_equal(mat, ref_imp), name
+    # caller buffers (extract_long_into): the spare rows stay untouched, a buffer one row short is refused
+    for name, o in orders.items():
+        out_ids, out = np.full(len(uid_ref) + 3, -99, np.int64), np.full((len(uid_ref) + 3, plan.n_cols), -99.0)
+        assert dp.extract_long_into(ids[o], t[o], v[o], out_ids, out) == len(uid_ref), name
+        assert np.array_equal(out_ids[:len(uid_ref)], uid_ref) and np.array_equal(out[:len(uid_ref)], ref, equal_nan=True)
+        assert (out_ids[len(uid_ref):] == -99).all() and (out[len(uid_ref):] == -99.0).all()
+        with pytest.raises(ValueError, match="out_capacity too small"):
+            dp.extract_long_into(ids[o], t[o], v[o], out_ids[:len(uid_ref) - 1], out[:len(uid_ref) - 1])
 
 
 def test_nan_values_are_an_error(env):
@@ -126,9 +156,12 @@ def test_extract_features_reports_the_nan_column():
         extraction._HOST_NAN_CHECK_ROWS = old
 
 
-def test_device_pointers(env):
+def test_device_rows_go_through_the_staged_calls(env):
+    """device rows of one kind, no kind codes: tsfx_stage_long_stacked + tsfx_extract_staged give the ids and matrix of the
+    host path; tsfx_extract_long refuses device pointers"""
     torch = pytest.importorskip("torch")
     import ctypes
+    import re
     from tsfresh_b200 import _lib
     ctx, dp, plan = env
     rng = np.random.default_rng(5)
@@ -137,17 +170,25 @@ def test_device_pointers(env):
     dev = torch.device("cuda", 0)
     for order in (np.arange(len(ids)), rng.permutation(len(ids))):
         d_ids, d_t, d_v = (torch.from_numpy(a[order]).to(dev) for a in (ids, t, v))
-        d_uid = torch.empty(len(uid_ref), dtype=torch.int64, device=dev)
-        d_out = torch.empty((len(uid_ref), plan.n_cols), dtype=torch.float64, device=dev)
-        n = ctypes.c_int64(0)
-        rc = ctx.lib.tsfx_extract_long(ctx.h, dp.h, ctypes.c_void_p(d_ids.data_ptr()), ctypes.c_void_p(d_t.data_ptr()), 0,
-                                       ctypes.c_void_p(d_v.data_ptr()), len(ids), ctypes.c_void_p(d_uid.data_ptr()),
-                                       ctypes.c_void_p(d_out.data_ptr()), len(uid_ref), ctypes.byref(n), _lib.FLAG_DEVICE_PTRS)
-        ctx.check(rc, "tsfx_extract_long")
+        torch.cuda.synchronize(dev)
+        n_ids, rows, max_len = ctx.stage_long_stacked(d_ids.data_ptr(), d_t.data_ptr(), 0, d_v.data_ptr(), 0, 0, 1, 0, len(ids))
+        assert n_ids == len(uid_ref) and rows[0] == len(ids) and max_len[0] == lens.max()
+        d_uid = torch.empty(n_ids, dtype=torch.int64, device=dev)
+        d_out = torch.empty((n_ids, plan.n_cols), dtype=torch.float64, device=dev)
+        ctx.extract_staged([dp], d_uid.data_ptr(), d_out.data_ptr(), plan.n_cols)
         ctx.sync()
-        assert n.value == len(uid_ref)
         assert np.array_equal(d_uid.cpu().numpy(), uid_ref)
         assert np.array_equal(d_out.cpu().numpy(), ref, equal_nan=True)
+    n = ctypes.c_int64(0)
+    rc = ctx.lib.tsfx_extract_long(ctx.h, dp.h, ctypes.c_void_p(d_ids.data_ptr()), ctypes.c_void_p(d_t.data_ptr()), 0,
+                                   ctypes.c_void_p(d_v.data_ptr()), len(ids), ctypes.c_void_p(d_uid.data_ptr()),
+                                   ctypes.c_void_p(d_out.data_ptr()), len(uid_ref), ctypes.byref(n), _lib.FLAG_DEVICE_PTRS)
+    assert rc == -1 and n.value == 0
+    msg = "tsfx_extract_long takes host pointers (device rows: tsfx_stage_long_stacked, tsfx_extract_staged)"
+    with pytest.raises(ValueError, match=re.escape(msg)):
+        ctx.check(rc, "tsfx_extract_long")
+    uid, mat = dp.extract_long(ids, t, v)                 # the context stays usable
+    assert np.array_equal(uid, uid_ref) and np.array_equal(mat, ref, equal_nan=True)
 
 
 def test_pinned_pool_reuses_blocks(env):

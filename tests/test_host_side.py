@@ -23,7 +23,7 @@ def test_library_exports_every_declared_symbol():
     lib = ctypes.CDLL(_lib.LIB_PATH) if os.path.exists(_lib.LIB_PATH) else _lib.load()
     for name in declared:
         assert hasattr(lib, name), name
-    assert _lib.load().tsfx_version() == 3
+    assert _lib.load().tsfx_version() == 4
 
 
 def test_plan_descriptor_table():

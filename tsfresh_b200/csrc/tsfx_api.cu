@@ -1162,16 +1162,15 @@ extern "C" int tsfx_kernel_variants(const char** names_out, int32_t cap) {
 }
 
 // ------------------------------------------------------------------------------------------ stage (a)
-// Long frame -> device CSR -> kernels, pipelined.  See tsfx_csr.h for the two paths.  `in` columns are host pointers
-// (copied through Stager::h2d: pinned sources go straight to cudaMemcpyAsync, pageable ones through the pinned ring)
-// or, with TSFX_FLAG_DEVICE_PTRS, device pointers that are used in place.
+// Long frame on the host -> device CSR -> kernels, pipelined.  See tsfx_csr.h for the two paths.  The columns are copied
+// through Stager::h2d (pinned sources go straight to cudaMemcpyAsync, pageable ones through the pinned ring) into the
+// workspace's W.ids() / W.keys() / W.vals(), and the value columns of kinds 1.. into ctx->kvals.
 struct LongIn {
     const int64_t* ids;
     const void* keys;
     int is_f64;
     const float* values;           // value column of kind 0
     int64_t n;
-    bool device;
     const float* const* more = nullptr;   // value columns of kinds 1 .. n_kinds-1 (wide format: the kinds share ids and sort keys)
     int n_kinds = 1;
     const float* col(int k) const { return k == 0 ? values : more[k - 1]; }
@@ -1181,52 +1180,37 @@ static inline size_t kind_stride(int64_t n) { return ((size_t)n + 3) & ~(size_t)
 
 static int nan_error(tsfx_ctx* ctx) { return fail(ctx, TSFX_E_NAN, "the value column contains NaN"); }
 
-// Brings the frame into CSR form on the device (sizes in *info).  When the rows arrive ordered and the input is on
-// the host, only the id column has been copied on return (*streamed = true): the caller streams the other columns.
-static int stage_a(tsfx_ctx* ctx, const LongIn& in, int max_blocks, bool check_nan, CsrInfo* info, bool* streamed,
-                   const int64_t** d_ids_out, const uint64_t** d_keys_out, const float** d_vals_out) {
+// Copies the id column to the device and runs the ids pass; one synchronisation for the sizes (*info).  The key and
+// value columns are then streamed by run_blocks (ids ascending) or copied whole by stage_a_sort.
+static int stage_a(tsfx_ctx* ctx, const LongIn& in, int max_blocks, CsrInfo* info) {
     CsrWorkspace& W = ctx->csr;
-    std::string msg;
     const int64_t n = in.n;
-    const int64_t* d_ids = in.ids;
-    const uint64_t* d_keys = (const uint64_t*)in.keys;
-    const float* d_vals = in.values;
-    if (!in.device) {
-        CK(W.reserve(0, (size_t)n * 8));
-        CK(W.reserve(2, (size_t)n * 4 + 16));
-        if (in.keys) CK(W.reserve(1, (size_t)n * 8));
-        CK(ctx->stager.h2d(W.ids(), in.ids, (size_t)n * 8, ctx->stream));
-        d_ids = W.ids();
-        d_keys = in.keys ? W.keys() : nullptr;
-        d_vals = W.vals();
-    }
-    int rc = csr_ids_pass(W, d_ids, n, 16384, max_blocks, ctx->stream, &msg);
+    CK(W.reserve(0, (size_t)n * 8));
+    CK(W.reserve(2, (size_t)n * 4 + 16));
+    if (in.keys) CK(W.reserve(1, (size_t)n * 8));
+    CK(ctx->stager.h2d(W.ids(), in.ids, (size_t)n * 8, ctx->stream));
+    std::string msg;
+    int rc = csr_ids_pass(W, W.ids(), n, 16384, max_blocks, ctx->stream, &msg);
     if (rc) return fail(ctx, rc, msg);
     CK(cudaStreamSynchronize(ctx->stream));
     *info = *W.h_info;
-    *streamed = false;
-    if (!info->unsorted_ids) {
-        W.d_values = const_cast<float*>(d_vals);
-        if (!in.device) *streamed = true;
-        else csr_check_rows(W, d_ids, d_keys, in.is_f64, d_vals, 0, n, check_nan, ctx->stream);   // result read by the caller
-    }
-    *d_ids_out = d_ids; *d_keys_out = d_keys; *d_vals_out = d_vals;
     return TSFX_OK;
 }
 
-// rows in arbitrary order: (copy the remaining columns,) sort, rebuild the CSR
-static int stage_a_sort(tsfx_ctx* ctx, const LongIn& in, int max_blocks, bool check_nan, CsrInfo* info,
-                        const int64_t* d_ids, const uint64_t* d_keys, const float* d_vals) {
+// rows in arbitrary order: (copy the key and value columns unless they are resident,) sort, rebuild the CSR
+static int stage_a_sort(tsfx_ctx* ctx, const LongIn& in, bool resident, int max_blocks, bool check_nan, CsrInfo* info) {
     CsrWorkspace& W = ctx->csr;
-    std::string msg;
-    if (!in.device) {
+    if (!resident) {
         if (in.keys) CK(ctx->stager.h2d(W.keys(), in.keys, (size_t)in.n * 8, ctx->stream));
         CK(ctx->stager.h2d(W.vals(), in.values, (size_t)in.n * 4, ctx->stream));
     }
-    int rc = csr_sort_pass(W, d_ids, d_keys, in.is_f64, d_vals, in.n, 16384, max_blocks, check_nan, ctx->stream, &msg);
+    std::string msg;
+    int rc = csr_sort_pass(W, W.ids(), in.keys ? W.keys() : nullptr, in.is_f64, W.vals(), in.n, 16384, max_blocks, check_nan,
+                           ctx->stream, &msg);
     if (rc) return fail(ctx, rc, msg);
     CK(cudaStreamSynchronize(ctx->stream));
     *info = *W.h_info;
+    if (info->has_nan) return nan_error(ctx);
     return TSFX_OK;
 }
 
@@ -1239,35 +1223,31 @@ struct KindSet {
     int total_cols = 0;
 };
 
-// kernels + result transfer over the row blocks of a device CSR.  stream_in: the key / value rows of a block are
-// copied from the host right before the block's kernels (fast path); d_out == nullptr: results go through ctx->out
-// and are copied to `out` (host) block by block on the D2H stream.  Several kinds (wide format) share the CSR: every
-// block runs each kind's plan on that kind's value column and writes its own column block of the one result matrix.
-static int run_blocks(tsfx_ctx* ctx, const KindSet& K, const CsrInfo& info, const LongIn* stream_in,
-                      const int64_t* d_ids, const uint64_t* d_keys, bool check_rows, bool check_nan,
-                      double* out, bool out_is_device, uint32_t flags, const int64_t* row_times = nullptr) {
+// kernels + result transfer over the row blocks of the device CSR: results go through ctx->out and are copied to `out`
+// (host) block by block on the D2H stream.  stream_in (rows ordered by id, only the ids on the device): the key / value
+// rows of a block are copied from the host right before the block's kernels and checked for sort keys that decrease
+// inside an id and for NaN.  Several kinds (wide format) share the CSR: every block runs each kind's plan on that kind's
+// value column and writes its own column block of the one result matrix.
+static int run_blocks(tsfx_ctx* ctx, const KindSet& K, const CsrInfo& info, const LongIn* stream_in, bool check_nan,
+                      double* out, uint32_t flags, const int64_t* row_times) {
     CsrWorkspace& W = ctx->csr;
     const size_t ncols = (size_t)K.total_cols;
     const int64_t ns = info.n_series;
-    double* dout = out;
-    if (!out_is_device) {
-        CK(ctx->out.reserve(std::max<size_t>((size_t)ns * ncols * sizeof(double), 8)));
-        dout = (double*)ctx->out.p;
-    }
+    CK(ctx->out.reserve(std::max<size_t>((size_t)ns * ncols * sizeof(double), 8)));
+    double* dout = (double*)ctx->out.p;
     const bool impute = (flags & TSFX_FLAG_IMPUTE) != 0;
     for (int b = 0; b < info.n_blocks; ++b) {
         const int64_t s0 = info.series_lo[b], s1 = info.series_lo[b + 1];
         const int64_t r0 = info.row_lo[b], r1 = info.row_lo[b + 1];
         const int slot = b & 1;
         if (stream_in) {
-            if (stream_in->keys) CK(ctx->stager.h2d(W.keys() + r0, (const uint64_t*)stream_in->keys + r0, (size_t)(r1 - r0) * 8, ctx->s_in));
+            const uint64_t* d_keys = stream_in->keys ? W.keys() : nullptr;
+            if (d_keys) CK(ctx->stager.h2d(W.keys() + r0, (const uint64_t*)stream_in->keys + r0, (size_t)(r1 - r0) * 8, ctx->s_in));
             for (int k = 0; k < K.n; ++k)
                 CK(ctx->stager.h2d(const_cast<float*>(K.dvals[k]) + r0, stream_in->col(k) + r0, (size_t)(r1 - r0) * 4, ctx->s_in));
             CK(cudaEventRecord(ctx->ev_in[slot], ctx->s_in));
             CK(cudaStreamWaitEvent(ctx->stream, ctx->ev_in[slot], 0));
-        }
-        if (check_rows) {
-            csr_check_rows(W, d_ids, d_keys, stream_in ? stream_in->is_f64 : 0, K.dvals[0], r0, r1, check_nan, ctx->stream);
+            csr_check_rows(W, W.ids(), d_keys, stream_in->is_f64, K.dvals[0], r0, r1, check_nan, ctx->stream);
             if (check_nan) for (int k = 1; k < K.n; ++k) csr_check_nan(W, K.dvals[k] + r0, r1 - r0, ctx->stream);
         }
         for (int k = 0; k < K.n; ++k) {
@@ -1278,7 +1258,7 @@ static int run_blocks(tsfx_ctx* ctx, const KindSet& K, const CsrInfo& info, cons
             int rc = run_groups(ctx, K.plan[k], R, info.max_len, dout + (size_t)s0 * ncols + K.col0[k], flags, K.total_cols);
             if (rc) return rc;
         }
-        if (impute || out_is_device) continue;
+        if (impute) continue;
         CK(cudaEventRecord(ctx->ev_done[slot], ctx->stream));
         CK(cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[slot], 0));
         CK(cudaMemcpyAsync(out + (size_t)s0 * ncols, dout + (size_t)s0 * ncols, (size_t)(s1 - s0) * ncols * sizeof(double),
@@ -1287,11 +1267,13 @@ static int run_blocks(tsfx_ctx* ctx, const KindSet& K, const CsrInfo& info, cons
     if (impute) {
         int rc = impute_after_extract(ctx, dout, ns, K.total_cols);
         if (rc) return rc;
-        if (!out_is_device) CK(cudaMemcpyAsync(out, dout, (size_t)ns * ncols * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(out, dout, (size_t)ns * ncols * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
     }
     return TSFX_OK;
 }
 
+// Rows with ascending ids take one streamed pass; if it finds a sort key that decreases inside an id, the columns it left
+// on the device are sorted and the kernels run again.  Rows in any other order are copied whole and sorted first.
 static int extract_long_impl(tsfx_ctx* ctx, const tsfx_plan* const* plans, const LongIn& in, int64_t* out_ids, double* out,
                              int64_t out_capacity, int64_t** out_ids_alloc, double** out_alloc, int64_t* n_series_out,
                              uint32_t flags) {
@@ -1308,95 +1290,82 @@ static int extract_long_impl(tsfx_ctx* ctx, const tsfx_plan* const* plans, const
     }
     for (int k = 0; k < K.n; ++k) if (plans[k]->need_times) plan = plans[k];      // take_times looks at one plan's flag
     const size_t kstride = kind_stride(in.n);
-    if (K.n > 1 && !in.device) CK(ctx->kvals.reserve((size_t)(K.n - 1) * kstride * 4 + 16));
+    if (K.n > 1) CK(ctx->kvals.reserve((size_t)(K.n - 1) * kstride * 4 + 16));
+    auto kind_in = [&](int k) { return (float*)ctx->kvals.p + (size_t)(k - 1) * kstride; };   // kind k >= 1, input row order
     const bool check_nan = !(flags & TSFX_FLAG_NO_NAN_CHECK);
     const int max_blocks = (flags & TSFX_FLAG_TIMING) ? 1 : 16;
     const int64_t* times_in = nullptr;           // row timestamps (input row order), device
     int rc = take_times(ctx, plan, in.n, &times_in);
     if (rc) return rc;
-    CsrInfo info;
-    bool streamed = false;
-    const int64_t* d_ids; const uint64_t* d_keys; const float* d_vals;
-    rc = stage_a(ctx, in, max_blocks, check_nan, &info, &streamed, &d_ids, &d_keys, &d_vals);
-    if (rc) return rc;
-    bool sorted = !info.unsorted_ids;
-    bool extra_resident = in.device;              // value columns of kinds 1.. are on the device in input order
-    auto extra_in = [&](int k) -> const float* {  // device column of kind k >= 1, input row order
-        return in.device ? in.col(k) : (const float*)ctx->kvals.p + (size_t)(k - 1) * kstride;
-    };
-    if (sorted && in.device && check_nan)
-        for (int k = 1; k < K.n; ++k) csr_check_nan(W, in.col(k), in.n, ctx->stream);
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        if (!sorted) {
-            rc = stage_a_sort(ctx, in, max_blocks, check_nan, &info, d_ids, d_keys, d_vals);
-            if (rc) return rc;
-            if (info.has_nan) return nan_error(ctx);
-        }
-        // device value column of every kind in CSR order
-        K.dvals[0] = W.d_values;
-        if (K.n > 1) {
-            if (W.d_perm) {                       // rows were sorted on the device: the other kinds follow the permutation
-                CK(ctx->kvals_sorted.reserve((size_t)(K.n - 1) * kstride * 4 + 16));
-                for (int k = 1; k < K.n; ++k) {
-                    if (!extra_resident) CK(ctx->stager.h2d(const_cast<float*>(extra_in(k)), in.col(k), (size_t)in.n * 4, ctx->stream));
-                    if (check_nan) csr_check_nan(W, extra_in(k), in.n, ctx->stream);
-                    float* dst = (float*)ctx->kvals_sorted.p + (size_t)(k - 1) * kstride;
-                    csr_gather_f32(W, extra_in(k), dst, in.n, ctx->stream);
-                    K.dvals[k] = dst;
-                }
-                extra_resident = true;
-            } else {
-                for (int k = 1; k < K.n; ++k) K.dvals[k] = extra_in(k);
-            }
-        }
+    // the result: blocks from the pinned pool (out_alloc) or the caller's buffers, once the number of series is known
+    auto size_result = [&](const CsrInfo& info) -> int {
         const int64_t ns = info.n_series;
         *n_series_out = ns;
-        const size_t ob = (size_t)ns * K.total_cols * sizeof(double);
-        if (out_alloc) {                         // library-sized result from the pinned pool
-            if (!*out_alloc) {
-                *out_alloc = (double*)ctx->pool.alloc(std::max<size_t>(ob, 8));
-                *out_ids_alloc = (int64_t*)ctx->pool.alloc(std::max<size_t>((size_t)ns * 8, 8));
-                if (!*out_alloc || !*out_ids_alloc) return fail(ctx, TSFX_E_NOMEM, "pinned host allocation failed");
-            }
+        if (out_alloc) {
+            *out_alloc = (double*)ctx->pool.alloc(std::max<size_t>((size_t)ns * K.total_cols * sizeof(double), 8));
+            *out_ids_alloc = (int64_t*)ctx->pool.alloc(std::max<size_t>((size_t)ns * 8, 8));
+            if (!*out_alloc || !*out_ids_alloc) return fail(ctx, TSFX_E_NOMEM, "pinned host allocation failed");
             out = *out_alloc;
             out_ids = *out_ids_alloc;
         } else if (ns > out_capacity) {
             return fail(ctx, TSFX_E_INVALID, "out_capacity too small: " + std::to_string(ns) + " series");
         }
         if (info.max_len < 1 && ns > 0) return fail(ctx, TSFX_E_INVALID, "empty series");
-        const bool first_sorted_try = sorted && attempt == 0;
-        const int64_t* row_times = times_in;
-        if (times_in && W.d_perm) {               // the rows were sorted on the device: the timestamps follow
-            CK(ctx->times_sorted.reserve((size_t)in.n * 8));
-            csr_gather_i64(W, times_in, (int64_t*)ctx->times_sorted.p, in.n, ctx->stream);
-            row_times = (const int64_t*)ctx->times_sorted.p;
-        }
-        rc = run_blocks(ctx, K, info, (first_sorted_try && streamed) ? &in : nullptr, d_ids, d_keys,
-                        /*check_rows=*/first_sorted_try && streamed, check_nan, out, in.device, flags, row_times);
-        if (first_sorted_try && streamed) extra_resident = true;
+        return TSFX_OK;
+    };
+    CsrInfo info;
+    rc = stage_a(ctx, in, max_blocks, &info);
+    if (rc) return rc;
+    bool streamed = false;         // the streamed pass ran: the result is sized and every column is on the device
+    if (!info.unsorted_ids) {
+        W.d_values = W.vals();
+        K.dvals[0] = W.d_values;
+        for (int k = 1; k < K.n; ++k) K.dvals[k] = kind_in(k);
+        rc = size_result(info);
         if (rc) return rc;
-        if (out_ids) CK(cudaMemcpyAsync(out_ids, W.d_uid, (size_t)ns * sizeof(int64_t), in.device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, ctx->stream));
-        if (in.device && !first_sorted_try) break;                       // asynchronous contract: nothing to wait for
-        // the NaN scans of the other kinds' columns were queued after the sort pass read its flags: read them again
-        const bool late_nan_flags = !first_sorted_try && K.n > 1 && check_nan;
-        if (first_sorted_try || late_nan_flags) CK(cudaMemcpyAsync(W.h_info, W.d_info, sizeof(CsrInfo), cudaMemcpyDeviceToHost, ctx->stream));
+        rc = run_blocks(ctx, K, info, &in, check_nan, out, flags, times_in);
+        if (rc) return rc;
+        if (out_ids) CK(cudaMemcpyAsync(out_ids, W.d_uid, (size_t)info.n_series * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaMemcpyAsync(W.h_info, W.d_info, sizeof(CsrInfo), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->s_out));
         CK(cudaStreamSynchronize(ctx->stream));
-        if (late_nan_flags && W.h_info->has_nan) return nan_error(ctx);
-        if (!first_sorted_try) break;
         if (W.h_info->has_nan) return nan_error(ctx);
-        if (!W.h_info->unsorted_keys) break;
-        // ids ascending but some sort key decreases inside an id: the columns are resident now, sort and run again
-        sorted = false;
-        if (!in.device) {
-            LongIn dev{d_ids, d_keys, in.is_f64, d_vals, in.n, true};
-            rc = stage_a_sort(ctx, dev, max_blocks, check_nan, &info, d_ids, d_keys, d_vals);
-            if (rc) return rc;
-            if (info.has_nan) return nan_error(ctx);
-            sorted = true;                        // CSR rebuilt: second trip only runs the kernels
-            streamed = false;
+        if (!W.h_info->unsorted_keys) return TSFX_OK;
+        streamed = true;           // some sort key decreases inside an id
+    }
+    rc = stage_a_sort(ctx, in, /*resident=*/streamed, max_blocks, check_nan, &info);
+    if (rc) return rc;
+    // the rows were sorted on the device: the other kinds and the row timestamps follow the permutation
+    K.dvals[0] = W.d_values;
+    if (K.n > 1) {
+        CK(ctx->kvals_sorted.reserve((size_t)(K.n - 1) * kstride * 4 + 16));
+        for (int k = 1; k < K.n; ++k) {
+            if (!streamed) CK(ctx->stager.h2d(kind_in(k), in.col(k), (size_t)in.n * 4, ctx->stream));
+            if (check_nan) csr_check_nan(W, kind_in(k), in.n, ctx->stream);
+            float* dst = (float*)ctx->kvals_sorted.p + (size_t)(k - 1) * kstride;
+            csr_gather_f32(W, kind_in(k), dst, in.n, ctx->stream);
+            K.dvals[k] = dst;
         }
     }
+    if (!streamed) {
+        rc = size_result(info);
+        if (rc) return rc;
+    }
+    const int64_t* row_times = nullptr;
+    if (times_in) {
+        CK(ctx->times_sorted.reserve((size_t)in.n * 8));
+        csr_gather_i64(W, times_in, (int64_t*)ctx->times_sorted.p, in.n, ctx->stream);
+        row_times = (const int64_t*)ctx->times_sorted.p;
+    }
+    rc = run_blocks(ctx, K, info, nullptr, check_nan, out, flags, row_times);
+    if (rc) return rc;
+    if (out_ids) CK(cudaMemcpyAsync(out_ids, W.d_uid, (size_t)info.n_series * sizeof(int64_t), cudaMemcpyDeviceToHost, ctx->stream));
+    // the NaN scans of the other kinds' columns were queued after the sort pass read its flags: read them again
+    const bool late_nan_flags = K.n > 1 && check_nan;
+    if (late_nan_flags) CK(cudaMemcpyAsync(W.h_info, W.d_info, sizeof(CsrInfo), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->s_out));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (late_nan_flags && W.h_info->has_nan) return nan_error(ctx);
     return TSFX_OK;
 }
 
@@ -1405,12 +1374,14 @@ extern "C" int tsfx_extract_long(tsfx_ctx* ctx, const tsfx_plan* plan, const int
                                  double* out, int64_t out_capacity, int64_t* n_series_out, uint32_t flags) {
     if (!ctx) return TSFX_E_INVALID;
     if (!plan || plan->ctx != ctx) return fail(ctx, TSFX_E_INVALID, "plan does not belong to this context");
+    if (flags & TSFX_FLAG_DEVICE_PTRS)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long takes host pointers (device rows: tsfx_stage_long_stacked, tsfx_extract_staged)");
     if (n_rows < 0 || !n_series_out || (n_rows > 0 && (!ids || !values)) || !out)
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long: bad arguments");
     CK(cudaSetDevice(ctx->device));
     *n_series_out = 0;
     if (n_rows == 0) return TSFX_OK;
-    LongIn in{ids, sort_keys, sort_key_is_f64, values, n_rows, (flags & TSFX_FLAG_DEVICE_PTRS) != 0};
+    LongIn in{ids, sort_keys, sort_key_is_f64, values, n_rows};
     return extract_long_impl(ctx, &plan, in, out_ids, out, out_capacity, nullptr, nullptr, n_series_out, flags);
 }
 
@@ -1440,7 +1411,7 @@ extern "C" int tsfx_extract_long_alloc(tsfx_ctx* ctx, const tsfx_plan* plan, con
     if (flags & TSFX_FLAG_DEVICE_PTRS) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_alloc takes host pointers");
     if (n_rows < 0 || !n_series_out || !out || !out_ids || (n_rows > 0 && (!ids || !values)))
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_alloc: bad arguments");
-    return extract_long_pooled(ctx, &plan, LongIn{ids, sort_keys, sort_key_is_f64, values, n_rows, false}, out_ids, out,
+    return extract_long_pooled(ctx, &plan, LongIn{ids, sort_keys, sort_key_is_f64, values, n_rows}, out_ids, out,
                                n_series_out, flags);
 }
 
@@ -1454,7 +1425,7 @@ extern "C" int tsfx_extract_long_kinds(tsfx_ctx* ctx, const tsfx_plan* const* pl
         return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_kinds: bad arguments");
     for (int k = 0; k < n_kinds; ++k)
         if (!plans[k] || (n_rows > 0 && !values[k])) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_kinds: NULL plan / column");
-    LongIn in{ids, sort_keys, sort_key_is_f64, values[0], n_rows, false};
+    LongIn in{ids, sort_keys, sort_key_is_f64, values[0], n_rows};
     in.more = values + 1;
     in.n_kinds = n_kinds;
     return extract_long_pooled(ctx, plans, in, out_ids, out, n_series_out, flags);

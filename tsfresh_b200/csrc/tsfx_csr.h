@@ -44,7 +44,7 @@ struct CsrWorkspace {
     void release();
     cudaError_t reserve(int slot, size_t bytes);
     cudaError_t init_info();
-    // device copies of the input columns (device-pointer callers alias their own buffers instead)
+    // device copies of the input columns (host-pointer stage (a): tsfx_extract_long[_alloc|_kinds])
     int64_t* ids() const { return (int64_t*)bufs[0]; }
     uint64_t* keys() const { return (uint64_t*)bufs[1]; }
     float* vals() const { return (float*)bufs[2]; }
