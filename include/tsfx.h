@@ -304,14 +304,30 @@ int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* o
  *                         entries; the exact longest window, which tsfx_extract_staged checks against each plan's
  *                         limit).  TSFX_E_INVALID when two windows of one kind have the same name (sort keys tied at
  *                         their naming rows; the reference would merge them into one series).  No feature kernel runs.
- *                         No flags are defined for it yet: pass 0.
+ *                         No flags are defined for it yet: pass 0.  TSFX_E_INVALID when the staged rows are already
+ *                         rolled or packaged (tsfx_sub_staged).
  *   tsfx_staged_row_keys  copies the naming sort keys (raw int64 / float64 bits as staged, float64 -0.0 as +0.0; row
  *                         numbers as int64 without sort keys) of the n_rows_out staged windows to out_keys (device, 8
- *                         bytes each), asynchronously.  Valid until the next stage call.
+ *                         bytes each), asynchronously.  Valid until the next stage call.  After tsfx_sub_staged it
+ *                         copies the package numbers (int64) of the staged packages instead.
  * tsfx_extract_staged then extracts the windows: out_ids receives the id of every union window. */
 int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                      int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags);
 int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys);
+
+/* Fixed-length packages of staged rows (extract_features(add_sub_time_series_index(df, sub_length, ...)),
+ * dataframe_functions.py:683-784), between tsfx_stage_long_stacked and tsfx_extract_staged:
+ *   tsfx_sub_staged       cuts every staged (kind, id) series, in (id, sort key) order, into packages of sub_length rows,
+ *                         the last one shorter: package k is rows [k * sub_length, min((k + 1) * sub_length, n)).  A
+ *                         package is a view on the staged values, so each kind keeps its row alignment.  A package is
+ *                         named (package number, parent id); the staged rows become the union of the names over all
+ *                         kinds, ascending in (package number, parent id).  Synchronises the stream once and returns the
+ *                         number of union packages in *n_rows_out and the longest package of every kind in
+ *                         max_len_per_kind (host, n_kinds entries; checked by tsfx_extract_staged against each plan's
+ *                         limit).  TSFX_E_INVALID for sub_length < 1, and when the staged rows are already rolled or
+ *                         packaged (stage them again).  No feature kernel runs.  No flags are defined for it yet: pass 0.
+ * tsfx_staged_row_keys then gives the package numbers (int64), and tsfx_extract_staged's out_ids the parent ids. */
+int tsfx_sub_staged(tsfx_ctx* ctx, int64_t sub_length, int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags);
 
 /* Page-locked host memory from the context's pool (freed blocks are cached: page-locking is slow). */
 void* tsfx_host_alloc(tsfx_ctx* ctx, size_t bytes);

@@ -39,7 +39,7 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
            "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged",
-           "tsfx_roll_staged", "tsfx_staged_row_keys"]
+           "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged"]
 
 
 def load():
@@ -92,6 +92,7 @@ def load():
         lib.tsfx_extract_staged.argtypes = [vp, vp, vp, vp, i32, u32]
         lib.tsfx_roll_staged.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i64), vp, u32]
         lib.tsfx_staged_row_keys.argtypes = [vp, vp]
+        lib.tsfx_sub_staged.argtypes = [vp, i64, ctypes.POINTER(i64), vp, u32]
         _lib = lib
         return lib
 
@@ -234,8 +235,18 @@ class Context:
         self.check(rc, "tsfx_roll_staged")
         return n_rows.value, max_len
 
+    def sub_staged(self, sub_length, n_kinds):
+        """tsfx_sub_staged: the staged series become their packages of sub_length rows.  Returns (number of union
+        packages, longest package of every kind).  Synchronises the context's stream once."""
+        n_rows = ctypes.c_int64(0)
+        max_len = np.zeros(n_kinds, dtype=np.int32)
+        rc = self.lib.tsfx_sub_staged(self.h, int(sub_length), ctypes.byref(n_rows), _ptr(max_len), 0)
+        self.check(rc, "tsfx_sub_staged")
+        return n_rows.value, max_len
+
     def staged_row_keys(self, keys_ptr):
-        """tsfx_staged_row_keys: the naming sort keys of the staged windows into device memory (8 bytes each)"""
+        """tsfx_staged_row_keys: the naming sort keys of the staged windows, or the package numbers of the staged
+        packages, into device memory (8 bytes each)"""
         self.check(self.lib.tsfx_staged_row_keys(self.h, ctypes.c_void_p(keys_ptr)), "tsfx_staged_row_keys")
 
     def extract_staged(self, device_plans, ids_ptr, out_ptr, ld, flags=0):

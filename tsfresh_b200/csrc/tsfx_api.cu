@@ -1457,6 +1457,7 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
     S.d_keys = nullptr;
     S.has_keys = false;
     S.rolled = false;
+    S.packaged = false;
     if (n_rows > 0) {
         std::string msg;
         int rc = stacked_stage(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values, kind_codes,
@@ -1548,7 +1549,8 @@ extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_
     StackedWorkspace& S = ctx->stacked;
     ctx->launches = 0;
     ctx->n_kernels = 0;
-    if (!S.valid || S.rolled) return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: no unrolled rows staged (tsfx_stage_long_stacked)");
+    if (!S.valid || S.rolled || S.packaged)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: no unrolled, unpackaged rows staged (tsfx_stage_long_stacked)");
     if (!n_rows_out || !max_len_per_kind || rolling_direction == 0 || max_timeshift < 0 || min_timeshift < 0)
         return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: bad arguments");
     if (S.has_keys && !S.d_keys)
@@ -1583,10 +1585,48 @@ extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_
     return TSFX_OK;
 }
 
+extern "C" int tsfx_sub_staged(tsfx_ctx* ctx, int64_t sub_length, int64_t* n_rows_out, int32_t* max_len_per_kind,
+                               uint32_t flags) {
+    (void)flags;
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (!S.valid || S.rolled || S.packaged)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_sub_staged: no unrolled, unpackaged rows staged (tsfx_stage_long_stacked)");
+    if (!n_rows_out || !max_len_per_kind || sub_length < 1) return fail(ctx, TSFX_E_INVALID, "tsfx_sub_staged: bad arguments");
+    S.valid = false;
+    *n_rows_out = 0;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
+    if (S.n_union == 0) { S.packaged = true; S.valid = true; return TSFX_OK; }
+    CK(cudaSetDevice(ctx->device));
+    const StackedInfo& I = *S.h_info;
+    // every series has fewer than 2^31 rows, so a longer sub_length gives the same packages: whole series
+    const int32_t L = (int32_t)std::min<int64_t>(sub_length, 0x7fffffff);
+    // a kind of r rows in s series has at most r / L full packages and one shorter package per series, and every
+    // package has a row
+    int64_t rows = 0, bound = 0;
+    for (int k = 0; k < S.n_kinds; ++k) {
+        rows += I.kind_rows[k];
+        bound += I.kind_rows[k] / L + (I.kind_series[k + 1] - I.kind_series[k]);
+    }
+    bound = std::min(bound, rows);
+    std::string msg;
+    int rc = stacked_sub(S, ctx->csr, L, bound, ctx->stream, &msg);
+    if (rc) return fail(ctx, rc, msg);
+    CK(cudaStreamSynchronize(ctx->stream));
+    S.n_union = I.n_union;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = I.kind_max_len[k];
+    *n_rows_out = S.n_union;
+    S.valid = true;
+    return TSFX_OK;
+}
+
 extern "C" int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys) {
     if (!ctx) return TSFX_E_INVALID;
     StackedWorkspace& S = ctx->stacked;
-    if (!S.rolled) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: no windows staged (tsfx_roll_staged)");
+    if (!S.rolled && !S.packaged)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: no windows or packages staged (tsfx_roll_staged, tsfx_sub_staged)");
     if (S.n_union == 0) return TSFX_OK;
     if (!out_keys) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: NULL out_keys");
     CK(cudaSetDevice(ctx->device));

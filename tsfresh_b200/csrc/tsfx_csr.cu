@@ -285,8 +285,10 @@ int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys,
 enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T_LEN, T_ROW, T_UID, T_INFO, T_KEYS,
        // stacked_roll: per-series window offsets, per-window begin / len / union row / parent id / name, scanned name
        // flags, union windows' names
-       R_OFF, R_BEGIN, R_LEN, R_ROW, R_ID, R_KEY, R_SCAN, R_UID, R_UKEY, T_SLOTS };
-static_assert(T_SLOTS <= 24, "StackedWorkspace::bufs");
+       R_OFF, R_BEGIN, R_LEN, R_ROW, R_ID, R_KEY, R_SCAN, R_UID, R_UKEY,
+       // stacked_sub: begin / len / union row of every package in union order inside its kind
+       P_BEGIN, P_LEN, P_ROW, T_SLOTS };
+static_assert(T_SLOTS <= 32, "StackedWorkspace::bufs");
 
 cudaError_t StackedWorkspace::reserve(int slot, size_t bytes) {
     if (bytes <= caps[slot]) return cudaSuccess;
@@ -309,7 +311,7 @@ void StackedWorkspace::release() {
     h_info = nullptr; d_info = nullptr;
     d_values = nullptr; d_times = nullptr; d_begin = nullptr; d_len = nullptr; d_row = nullptr; d_uid = nullptr;
     d_keys = nullptr; d_ukey = nullptr;
-    valid = false; rolled = false;
+    valid = false; rolled = false; packaged = false;
 }
 
 #define STACK_TILE 4096          // rows per CTA of the counting sort
@@ -468,6 +470,7 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
                   int64_t n, bool keep_keys, cudaStream_t st, std::string* msg) {
     S.valid = false;
     S.rolled = false;
+    S.packaged = false;
     S.n_kinds = n_kinds;
     S.has_keys = d_keys != nullptr;
     S.keys_f64 = d_keys && keys_f64;
@@ -704,6 +707,150 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
     S.d_len = wlen;
     S.d_row = wrow;
     S.rolled = true;
+    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
+    return TSFX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// fixed-length packages of the staged series (stacked_sub)
+
+// packages of every series into cnt[s]; each kind's longest package (its longest series, cut at L) into
+// info->kind_max_len (zeroed by the caller)
+__global__ void k_sub_count(const int32_t* __restrict__ len, int64_t n_series, int32_t L, int n_kinds,
+                            int32_t* __restrict__ cnt, StackedInfo* info) {
+    __shared__ int mx[TSFX_MAX_KINDS];
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) mx[k] = 0;
+    __syncthreads();
+    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; s < n_series; s += stride) {
+        const int32_t n = len[s];
+        cnt[s] = n / L + (n % L != 0);
+        if (n > 0) atomicMax(&mx[kind_of_series(info, n_kinds, s)], min(n, L));
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
+}
+
+// Sort key of package slot i that puts every kind's packages in the order of their union rows: (kind, union row), or
+// INT64_MAX for the slots from *n_packages on.  Reads the kinds' package ranges (info->kind_series after k_roll_kinds).
+__global__ void k_sub_layout_key(const int32_t* __restrict__ prow, const int32_t* __restrict__ n_packages, int64_t bound,
+                                 int n_kinds, const StackedInfo* info, int64_t* __restrict__ key) {
+    const int64_t np = *n_packages;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (const int64_t stride = (int64_t)gridDim.x * blockDim.x; i < bound; i += stride)
+        key[i] = i < np ? ((int64_t)kind_of_series(info, n_kinds, i) << 32) | prow[i] : INT64_MAX;
+}
+
+// package slot i takes the package perm[i]
+__global__ void k_sub_gather(const uint32_t* __restrict__ perm, const int32_t* __restrict__ n_packages,
+                             const int64_t* __restrict__ begin, const int32_t* __restrict__ len, const int32_t* __restrict__ row,
+                             int64_t* __restrict__ obegin, int32_t* __restrict__ olen, int32_t* __restrict__ orow) {
+    const int64_t np = *n_packages;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (const int64_t stride = (int64_t)gridDim.x * blockDim.x; i < np; i += stride) {
+        const uint32_t p = perm[i];
+        obegin[i] = begin[p];
+        olen[i] = len[p];
+        orow[i] = row[p];
+    }
+}
+
+// One warp per series, one lane per package: package j is rows [j * L, min((j + 1) * L, n)) of the series, named
+// (package number j, parent id).  The slots [off[n_series], bound) get the name that sorts after every real one
+// (INT64_MAX, INT64_MAX).
+__global__ void k_sub_fill(const int64_t* __restrict__ begin, const int32_t* __restrict__ len, const int32_t* __restrict__ row,
+                           const int64_t* __restrict__ uid, const int32_t* __restrict__ off, int64_t n_series, int64_t bound,
+                           int32_t L, int64_t* __restrict__ pbegin, int32_t* __restrict__ plen, int64_t* __restrict__ pid,
+                           int64_t* __restrict__ pnum) {
+    const int lane = threadIdx.x & 31;
+    int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (; s < n_series; s += n_warps) {                  // warp-uniform
+        const int64_t b = begin[s];
+        const int32_t n = len[s];
+        const int64_t id = uid[row[s]];
+        const int32_t o = off[s], np = off[s + 1] - o;
+        for (int32_t j = lane; j < np; j += 32) {
+            const int64_t lo = (int64_t)j * L;
+            pbegin[o + j] = b + lo;
+            plen[o + j] = (int32_t)min((int64_t)L, n - lo);
+            pid[o + j] = id;
+            pnum[o + j] = j;
+        }
+    }
+    int64_t i = off[n_series] + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    for (const int64_t stride = (int64_t)gridDim.x * blockDim.x; i < bound; i += stride) {
+        pid[i] = INT64_MAX;
+        pnum[i] = INT64_MAX;
+    }
+}
+
+int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, cudaStream_t st, std::string* msg) {
+    const int n_kinds = S.n_kinds;
+    const int64_t ns = S.h_info->kind_series[n_kinds];
+    const size_t nb = (size_t)std::max<int64_t>(bound, 1);
+    CKE(S.reserve(R_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
+    CKE(S.reserve(R_BEGIN, nb * 8), "alloc packages");
+    CKE(S.reserve(R_LEN, nb * 4), "alloc packages");
+    CKE(S.reserve(R_ROW, nb * 4), "alloc packages");
+    CKE(S.reserve(R_ID, nb * 8), "alloc packages");
+    CKE(S.reserve(R_KEY, nb * 8), "alloc packages");
+    CKE(S.reserve(R_SCAN, nb * 4), "alloc packages");
+    CKE(S.reserve(R_UID, nb * 8), "alloc packages");
+    CKE(S.reserve(R_UKEY, nb * 8), "alloc packages");
+    CKE(S.reserve(P_BEGIN, nb * 8), "alloc packages");
+    CKE(S.reserve(P_LEN, nb * 4), "alloc packages");
+    CKE(S.reserve(P_ROW, nb * 4), "alloc packages");
+    int32_t* off = (int32_t*)S.bufs[R_OFF];
+    int64_t* pbegin = (int64_t*)S.bufs[R_BEGIN];
+    int32_t* plen = (int32_t*)S.bufs[R_LEN];
+    int32_t* prow = (int32_t*)S.bufs[R_ROW];
+    int64_t* pid = (int64_t*)S.bufs[R_ID];
+    int64_t* pnum = (int64_t*)S.bufs[R_KEY];
+    int32_t* scan = (int32_t*)S.bufs[R_SCAN];
+    uint32_t* perm = nullptr;
+    size_t tb1 = 0, tb2 = 0;
+    NameChange change{pid, (const uint64_t*)pnum, nullptr, off + ns};
+    thrust::counting_iterator<int64_t> rows(0);
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb1, off, off, (int)(ns + 1), st), "scan size");
+    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st), "scan size");
+    CKE(S.reserve(T_TEMP, std::max(tb1, tb2)), "alloc temp");
+    // packages per series, their offsets, each kind's longest package
+    CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
+        "memset info");
+    CKE(cudaMemsetAsync(off + ns, 0, 4, st), "memset offsets");
+    k_sub_count<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, L, n_kinds, off, S.d_info);
+    CKE(cudaGetLastError(), "package count kernel");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb1, off, off, (int)(ns + 1), st), "package offsets");
+    k_sub_fill<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(S.d_begin, S.d_len, S.d_row, S.d_uid, off, ns,
+                                                                                 bound, L, pbegin, plen, pid, pnum);
+    CKE(cudaGetLastError(), "package fill kernel");
+    // the union of the names: sort (package number, parent id), flag and scan the distinct pairs
+    if (int rc = sort_rows(W, pnum, (const uint64_t*)pid, 0, bound, st, msg, &perm)) return rc;
+    change.perm = perm;
+    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st),
+        "union rows");
+    S.d_uid = (int64_t*)S.bufs[R_UID];
+    S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
+    k_roll_union<<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, pid, (const uint64_t*)pnum, prow, S.d_uid,
+                                                       S.d_ukey, S.d_info);
+    k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
+    CKE(cudaGetLastError(), "union kernels");
+    // The packages were filled series by series, (parent id, package number) order inside a kind, but the union rows
+    // ascend in (package number, parent id).  Reorder every kind's packages by union row, so that a kind with a package
+    // for every union row fills its columns in place, as tsfx_extract_staged expects.  The names are no longer needed:
+    // the sort key goes into their storage.
+    int64_t* key = pnum;
+    k_sub_layout_key<<<grid_for(bound, 256), 256, 0, st>>>(prow, off + ns, bound, n_kinds, S.d_info, key);
+    CKE(cudaGetLastError(), "package layout kernel");
+    if (int rc = sort_rows(W, key, nullptr, 0, bound, st, msg, &perm)) return rc;
+    S.d_begin = (int64_t*)S.bufs[P_BEGIN];
+    S.d_len = (int32_t*)S.bufs[P_LEN];
+    S.d_row = (int32_t*)S.bufs[P_ROW];
+    k_sub_gather<<<grid_for(bound, 256), 256, 0, st>>>(perm, off + ns, pbegin, plen, prow, S.d_begin, S.d_len, S.d_row);
+    CKE(cudaGetLastError(), "package gather kernel");
+    S.packaged = true;
     CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
     return TSFX_OK;
 }

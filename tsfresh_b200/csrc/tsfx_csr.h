@@ -109,9 +109,11 @@ struct StackedWorkspace {
     int64_t* d_begin = nullptr;   // series s = d_values[d_begin[s] .. + d_len[s])
     int32_t* d_len = nullptr;
     int32_t* d_row = nullptr;     // union row of series s
-    int64_t* d_uid = nullptr;     // union ids, ascending (keep_ids); after stacked_roll the parent id of every window
+    int64_t* d_uid = nullptr;     // union ids, ascending (keep_ids); after stacked_roll / stacked_sub the parent id of
+                                  // every union window / package
     uint64_t* d_keys = nullptr;   // sort keys (raw bits) in the order of d_values (stacked_stage with keep_keys)
-    uint64_t* d_ukey = nullptr;   // after stacked_roll: naming sort key of every union window (raw bits)
+    uint64_t* d_ukey = nullptr;   // after stacked_roll: naming sort key of every union window (raw bits); after
+                                  // stacked_sub: package number of every union package (int64)
     StackedInfo* h_info = nullptr;   // pinned
     StackedInfo* d_info = nullptr;
     int n_kinds = 0;
@@ -120,8 +122,9 @@ struct StackedWorkspace {
     bool has_keys = false;        // the rows came with sort keys
     bool keys_f64 = false;        //   float64 ones
     bool rolled = false;          // the staged series have been turned into windows (stacked_roll)
-    void* bufs[24] = {nullptr};
-    size_t caps[24] = {0};
+    bool packaged = false;        // the staged series have been cut into packages (stacked_sub)
+    void* bufs[32] = {nullptr};
+    size_t caps[32] = {0};
     cudaError_t reserve(int slot, size_t bytes);
     cudaError_t keep_ids(const int64_t* d_src, int64_t n, cudaStream_t st);   // d_uid = a copy of n union ids
     void release();
@@ -144,6 +147,14 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
 // Lmax = the longest staged series (the shifts' anchor); bound >= the number of windows.
 int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                  int32_t Lmax, int64_t bound, cudaStream_t st, std::string* msg);
+
+// Fixed-length packages (add_sub_time_series_index) of the staged series, as new staged series: package j of a series
+// of n rows is the view on its rows [j * L, min((j + 1) * L, n)), so each kind keeps its aligned rows.  Same structure as
+// stacked_roll (count, scan, fill with one warp per series, sort_rows over the names, flag and scan); a package is named
+// (package number, parent id) and the union rows ascend in that order.  d_uid / d_ukey get the parent id / package
+// number of every union row; d_info the package ranges of the kinds, their longest packages and n_union, copied to
+// h_info (the caller synchronises).  bound >= the number of packages.
+int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, cudaStream_t st, std::string* msg);
 
 // out[r * ld + c] = NaN for r < n_rows, c < n_cols
 cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cudaStream_t st);

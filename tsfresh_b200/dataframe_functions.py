@@ -9,6 +9,9 @@
 
 The matrix goes to the GPU as one row-major float64 block; `extract_features(impute_function=impute)` skips that
 round trip and imputes the feature matrix while it is still on the device (TSFX_FLAG_IMPUTE).
+
+    add_sub_time_series_index(df, sub_length, ...)   cuts every series into packages of sub_length rows (:683-784);
+                                                     pandas only (extract_features_sub_device does it on the device)
 """
 import warnings
 
@@ -93,3 +96,62 @@ def _warn_non_finite(df, m, stats, check_input=False):
         if bad.any():
             warnings.warn("The columns {} did not have any finite values. Filling with zeros.".format(
                 df.columns[np.where(zero)[0][bad]].values), RuntimeWarning)
+
+
+def _check_sub_length(sizes, sub_length):
+    """The exceptions add_sub_time_series_index (dataframe_functions.py:683-784) raises for a sub_length that cannot cut
+    series of these sizes (in group order): TypeError for a non-number, ZeroDivisionError for 0, ValueError when a
+    package count would be negative, AssertionError when the packages would not cover a series exactly."""
+    for n in sizes:
+        n = int(n)
+        q, r = divmod(n, sub_length)
+        if r < 0:
+            raise ValueError("negative dimensions are not allowed")
+        if n and (q < 0 or q * sub_length + r != n or sub_length != int(sub_length)):
+            raise AssertionError("packages of %r rows do not cover a series of %d rows" % (sub_length, n))
+        if sub_length > 0 and sub_length == int(sub_length):
+            return                          # a positive whole length cuts every series
+
+
+def add_sub_time_series_index(df_or_dict, sub_length, column_id=None, column_sort=None, column_kind=None):
+    """dataframe_functions.py:683-784: adds a column "id" that cuts every series into consecutive packages of sub_length
+    rows, the last one shorter.
+
+    A series is every (column_id, column_kind) group (groups without a key are dropped), or every column_kind group, or
+    the whole frame; its rows are taken in column_sort order, or in frame order without column_sort.  The package number
+    of row i of a series is i // sub_length.  "id" holds the package number, or the tuple (package number, column_id
+    value) with column_id; an existing "id" column is replaced.  The rows come grouped (groups ascending) with the key
+    columns moved behind the others, then sorted by column_sort when it is given; the frame's index labels are kept.
+    Unlike the reference, the input frame is never modified.  Rows with equal sort keys keep their frame order.
+
+    A dict of frames (already split by kind) is handled frame by frame; with column_kind it raises ValueError."""
+    if isinstance(df_or_dict, dict):
+        if column_kind is not None:
+            raise ValueError("You passed in a dictionary and gave a column name for the kind. Both are not possible.")
+        return {key: add_sub_time_series_index(frame, sub_length, column_id=column_id, column_sort=column_sort)
+                for key, frame in df_or_dict.items()}
+    df = df_or_dict
+    grouper = [c for c in (column_id, column_kind) if c is not None]
+    sort = None if column_sort is None else df[column_sort].to_numpy()
+    if grouper:
+        group = df.groupby(grouper, sort=True).ngroup().to_numpy()
+        columns = [c for c in df.columns if c not in grouper] + grouper
+    else:
+        group = np.zeros(len(df), dtype=np.int64)
+        columns = list(df.columns)
+    keep = np.flatnonzero(group >= 0)
+    if grouper and len(keep) == 0:
+        return df[columns[:len(columns) - len(grouper)]].iloc[:0]
+    # rows group by group (input order inside a group), then by sort key inside each group
+    order = pd.DataFrame({"g": group[keep]} if sort is None else {"g": group[keep], "s": sort[keep]})
+    order = keep[order.sort_values(list(order.columns), kind="stable").index.to_numpy()]
+    g = group[order]
+    starts = np.flatnonzero(np.r_[True, g[1:] != g[:-1]]) if len(g) else np.zeros(0, np.int64)
+    _check_sub_length(np.diff(np.r_[starts, len(g)]), sub_length)
+    rank = np.arange(len(g)) - np.repeat(starts, np.diff(np.r_[starts, len(g)]))
+    package = rank // sub_length
+    out = df.iloc[order][columns]
+    out["id"] = list(zip(package, out[column_id])) if column_id is not None else package
+    if column_sort is not None:
+        out = out.sort_values(column_sort)
+    return out

@@ -22,7 +22,15 @@ and torch then allocates the result that the extraction (tsfx_extract_staged) fi
 is extract_features(roll_time_series(frame, ...)) for the same rows: between the two calls, tsfx_roll_staged turns the
 staged series into their rolled windows (views on the staged values) and their union of names, with a second host
 synchronisation to learn the number of windows.
+
+    X, package_numbers, package_ids, columns = extract_features_sub_device(ids, values, sort, kind, kinds=[...],
+                                                                           sub_length=1000)
+
+is extract_features(add_sub_time_series_index(frame, 1000, ...), column_id="id") for the same rows: tsfx_sub_staged
+cuts the staged series into consecutive packages of sub_length rows (views again), named (package number, parent id).
 """
+import numbers
+
 import numpy as np
 import pandas as pd
 
@@ -171,12 +179,13 @@ def extract_features_device(values, begin=None, length=None, *, default_fc_param
     return X, columns
 
 
-def _long_layout(ids, values, sort, kind, kinds, times):
-    """(number of rows, kind names) of long-format row tensors from their shapes and dtypes alone (no device needed)."""
+def _long_layout(ids, values, sort, kind, kinds, times, need_ids=True):
+    """(number of rows, kind names) of long-format row tensors from their shapes and dtypes alone (no device needed).
+    need_ids=False: ids may be None (every row belongs to one id)."""
     import torch
     columns = (("ids", ids), ("values", values), ("sort", sort), ("kind", kind), ("times", times))
     for name, t in columns:
-        if t is None and name in ("ids", "values"):
+        if t is None and (name == "values" or (name == "ids" and need_ids)):
             raise TypeError("%s must be a torch.Tensor, not None" % name)
         if t is None:
             continue
@@ -184,7 +193,7 @@ def _long_layout(ids, values, sort, kind, kinds, times):
             raise TypeError("%s must be a torch.Tensor, not %s" % (name, type(t).__name__))
         if t.ndim != 1:
             raise ValueError("%s must be 1-D, got shape %s" % (name, tuple(t.shape)))
-    if ids.dtype != torch.int64:
+    if ids is not None and ids.dtype != torch.int64:
         raise TypeError("ids must be int64, not %s" % ids.dtype)
     if values.dtype not in (torch.float32, torch.float64, torch.float16, torch.bfloat16):
         raise TypeError("values must be float32, float64, float16 or bfloat16, not %s" % values.dtype)
@@ -194,10 +203,10 @@ def _long_layout(ids, values, sort, kind, kinds, times):
         raise TypeError("kind must be int32 or int64, not %s" % kind.dtype)
     if times is not None and times.dtype != torch.int64:
         raise TypeError("times must be int64 nanoseconds, not %s" % times.dtype)
-    n = ids.shape[0]
+    n, by = (values.shape[0], "values") if ids is None else (ids.shape[0], "ids")
     for name, t in columns[1:]:
         if t is not None and t.shape[0] != n:
-            raise ValueError("%s has %d rows, ids %d" % (name, t.shape[0], n))
+            raise ValueError("%s has %d rows, %s %d" % (name, t.shape[0], by, n))
     if n > (1 << 31) - 2 - 64 * 64:
         raise ValueError("%d rows: at most 2^31 - 4 098 in one call" % n)
     if kind is None:
@@ -281,13 +290,53 @@ def extract_features_rolled_device(ids, values, sort=None, kind=None, *, kinds=N
                            impute_function)
 
 
+def _sub_length(sub_length):
+    """add_sub_time_series_index's exception types for a sub_length it cannot package with (TypeError for a non-number,
+    ZeroDivisionError for 0, AssertionError for a negative or fractional length); then the length as int"""
+    if not isinstance(sub_length, numbers.Real):
+        raise TypeError("unsupported operand type(s) for //: 'int' and '%s'" % type(sub_length).__name__)
+    if sub_length == 0:
+        raise ZeroDivisionError("integer division or modulo by zero")
+    if not sub_length > 0 or sub_length != int(sub_length):
+        raise AssertionError("sub_length must be a positive integer, got %r" % (sub_length,))
+    return min(int(sub_length), (1 << 63) - 1)
+
+
+def extract_features_sub_device(ids, values, sort=None, kind=None, *, kinds=None, sub_length, times=None,
+                                default_fc_parameters=None, kind_to_fc_parameters=None, impute_function=None):
+    """Extracts features from fixed-length packages of long-format rows held in CUDA tensors into a CUDA tensor.
+
+    ids, values, sort, kind, kinds, times, default_fc_parameters, kind_to_fc_parameters and impute_function: as
+    extract_features_long_device, except that ids may be None: every kind is then one series, as with column_id=None.
+    sub_length: as add_sub_time_series_index.
+
+    Returns (X, package_numbers, package_ids, columns), what extract_features returns for add_sub_time_series_index(df,
+    sub_length, column_id="id", column_sort="time", column_kind="kind") of the equivalent frame, extracted with
+    column_id="id": every (id, kind) series, in sort order, is cut into packages of sub_length rows, the last one
+    shorter, and row r of X is the package named (package_numbers[r], package_ids[r]) (both int64; package_ids is None
+    without ids), names ascending, package number first.  The rows are the union of the package names over all kinds,
+    NaN where a kind has no package of that name.  The quadratic entropies' length limit applies to each package, not to
+    the series it comes from.
+
+    Runs on torch's current stream and blocks the host twice: to group the rows and to count the packages.  Raises
+    add_sub_time_series_index's exception types for a bad sub_length before the device is touched, and ValueError for
+    NaN values or sort keys, kind codes out of range and packages longer than their kind's plan allows, before any
+    feature kernel runs."""
+    L = _sub_length(sub_length)
+    X, package_ids, package_numbers, columns = _extract_staged(ids, values, sort, kind, kinds, times, None,
+                                                               default_fc_parameters, kind_to_fc_parameters,
+                                                               impute_function, sub_length=L)
+    return X, package_numbers, package_ids if ids is not None else None, columns
+
+
 def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_parameters, kind_to_fc_parameters,
-                    impute_function):
+                    impute_function, sub_length=None):
     """(X, row ids, row keys, columns) of long-format rows, staged by kind and extracted; with roll = (direction,
-    max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows' naming keys,
-    else None)."""
+    max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows' naming keys),
+    with sub_length they are cut into packages first (row keys: the package numbers; ids may then be None), else row
+    keys is None."""
     import torch
-    n, kinds = _long_layout(ids, values, sort, kind, kinds, times)
+    n, kinds = _long_layout(ids, values, sort, kind, kinds, times, need_ids=sub_length is None)
     if roll is not None and n <= 1:
         raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
     default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
@@ -303,7 +352,7 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
     row_keys = None
     with torch.cuda.device(dev):
         v = values.contiguous() if values.dtype == torch.float32 else values.to(torch.float32).contiguous()
-        i = ids.contiguous()
+        i = torch.zeros(n, dtype=torch.int64, device=dev) if ids is None else ids.contiguous()
         s = None if sort is None else sort.contiguous()
         k = None if kind is None else kind.contiguous()
         t = None if times is None else times.contiguous()
@@ -319,6 +368,10 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
                 if roll is not None:
                     n_rows, _ = ctx.roll_staged(*roll, len(kinds))
                     row_keys = torch.empty(n_rows, dtype=torch.int64 if s is None else s.dtype, device=dev)
+                    ctx.staged_row_keys(row_keys.data_ptr())
+                elif sub_length is not None:
+                    n_rows, _ = ctx.sub_staged(sub_length, len(kinds))
+                    row_keys = torch.empty(n_rows, dtype=torch.int64, device=dev)
                     ctx.staged_row_keys(row_keys.data_ptr())
                 present = [c for c in range(len(kinds)) if rows[c] > 0]
                 columns = [name for c in present for name in plans[c][1]]
