@@ -64,6 +64,9 @@ extern "C" {
                                   * so tsfx_last_launch_count is 0 after such an error. */
 #define TSFX_FLAG_KEEP_SORT_KEYS 64u /* tsfx_stage_long_stacked: keep every staged row's sort key, which tsfx_roll_staged
                                   * names its windows by (without the flag the call does no extra work) */
+#define TSFX_FLAG_KEEP_ROW_NUMBERS 128u /* tsfx_stage_long_stacked: keep every staged row's input row number (4 bytes per row),
+                                  * which tsfx_roll_staged with TSFX_FLAG_FORECAST finds the targets by */
+#define TSFX_FLAG_FORECAST 256u  /* tsfx_roll_staged: make_forecasting_frame's windows (see tsfx_staged_targets) */
 
 /* tsfx_impute modes (tsfresh/utilities/dataframe_functions.py) */
 #define TSFX_IMPUTE_RANGE 0      /* impute :49-78: +inf -> max, -inf -> min, NaN -> median of the finite values */
@@ -304,7 +307,7 @@ int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* o
  *                         entries; the exact longest window, which tsfx_extract_staged checks against each plan's
  *                         limit).  TSFX_E_INVALID when two windows of one kind have the same name (sort keys tied at
  *                         their naming rows; the reference would merge them into one series).  No feature kernel runs.
- *                         No flags are defined for it yet: pass 0.  TSFX_E_INVALID when the staged rows are already
+ *                         flags: 0, or TSFX_FLAG_FORECAST (below).  TSFX_E_INVALID when the staged rows are already
  *                         rolled or packaged (tsfx_sub_staged).
  *   tsfx_staged_row_keys  copies the naming sort keys (raw int64 / float64 bits as staged, float64 -0.0 as +0.0; row
  *                         numbers as int64 without sort keys) of the n_rows_out staged windows to out_keys (device, 8
@@ -314,6 +317,22 @@ int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans, int64_t* o
 int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                      int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags);
 int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys);
+
+/* Forecasting windows (make_forecasting_frame, dataframe_functions.py:606-680): tsfx_roll_staged with TSFX_FLAG_FORECAST,
+ * on rows staged with TSFX_FLAG_KEEP_ROW_NUMBERS (else TSFX_E_INVALID), rolls as above and then drops every window's last
+ * row, leaving out the windows that this empties (those of one row; the kept windows have at least
+ * max(min_timeshift, 1) + 1 rows before the drop).  Names, union rows and the one synchronisation are as without the flag;
+ * max_len_per_kind is the longest window after the drop.  Two windows of one kind with the same name are TSFX_E_INVALID
+ * as without the flag, counting the one-row windows that the drop empties: the reference names them too and merges each
+ * with a window of the same name before it drops a row.
+ *   tsfx_staged_targets   copies the target of each of the n_rows_out staged windows to out_rows (device, int64),
+ *                         asynchronously: the input row number of the row that names the window (the row the window
+ *                         forecasts is that row's value), or -1 when that is input row 0 (the reference's y = x[1:] has
+ *                         no entry for it).  A union row that several kinds' windows share takes the target of its
+ *                         lowest kind's window.  TSFX_E_INVALID unless the last roll had TSFX_FLAG_FORECAST; valid until
+ *                         the next stage call.
+ * The targets are row numbers, so the caller gathers the target values from its own copy of the input in any dtype. */
+int tsfx_staged_targets(tsfx_ctx* ctx, int64_t* out_rows);
 
 /* Fixed-length packages of staged rows (extract_features(add_sub_time_series_index(df, sub_length, ...)),
  * dataframe_functions.py:683-784), between tsfx_stage_long_stacked and tsfx_extract_staged:

@@ -19,6 +19,8 @@ FLAG_IMPUTE = 8
 FLAG_ALL_MEDIANS = 16
 FLAG_CHECK_DEVICE_INPUT = 32
 FLAG_KEEP_SORT_KEYS = 64
+FLAG_KEEP_ROW_NUMBERS = 128
+FLAG_FORECAST = 256
 STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy default stream for tsfx_ctx_set_stream
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
@@ -39,7 +41,7 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
            "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged",
-           "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged"]
+           "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged", "tsfx_staged_targets"]
 
 
 def load():
@@ -93,6 +95,7 @@ def load():
         lib.tsfx_roll_staged.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i64), vp, u32]
         lib.tsfx_staged_row_keys.argtypes = [vp, vp]
         lib.tsfx_sub_staged.argtypes = [vp, i64, ctypes.POINTER(i64), vp, u32]
+        lib.tsfx_staged_targets.argtypes = [vp, vp]
         _lib = lib
         return lib
 
@@ -210,10 +213,11 @@ class Context:
         return stats
 
     def stage_long_stacked(self, ids_ptr, sort_ptr, sort_is_f64, values_ptr, kind_ptr, kind_is_i64, n_kinds, times_ptr,
-                           n_rows, keep_sort_keys=False):
+                           n_rows, keep_sort_keys=False, keep_row_numbers=False):
         """tsfx_stage_long_stacked on device rows (pointers as ints, 0 for an absent column): returns (number of union
         ids, rows of every kind, longest series of every kind).  Synchronises the context's stream once.
-        keep_sort_keys: keep the sort keys for roll_staged."""
+        keep_sort_keys: keep the sort keys for roll_staged.  keep_row_numbers: keep the input row numbers for
+        roll_staged(forecast=True)."""
         n_ids = ctypes.c_int64(0)
         rows = np.zeros(n_kinds, dtype=np.int64)
         max_len = np.zeros(n_kinds, dtype=np.int32)
@@ -221,17 +225,19 @@ class Context:
                                               int(sort_is_f64), ctypes.c_void_p(values_ptr), ctypes.c_void_p(kind_ptr or None),
                                               int(kind_is_i64), int(n_kinds), ctypes.c_void_p(times_ptr or None), int(n_rows),
                                               ctypes.byref(n_ids), _ptr(rows), _ptr(max_len),
-                                              FLAG_DEVICE_PTRS | (FLAG_KEEP_SORT_KEYS if keep_sort_keys else 0))
+                                              FLAG_DEVICE_PTRS | (FLAG_KEEP_SORT_KEYS if keep_sort_keys else 0)
+                                              | (FLAG_KEEP_ROW_NUMBERS if keep_row_numbers else 0))
         self.check(rc, "tsfx_stage_long_stacked")
         return n_ids.value, rows, max_len
 
-    def roll_staged(self, rolling_direction, max_timeshift, min_timeshift, n_kinds):
-        """tsfx_roll_staged: the staged series become their rolled windows (max_timeshift 0: None).  Returns (number of
-        union windows, longest window of every kind).  Synchronises the context's stream once."""
+    def roll_staged(self, rolling_direction, max_timeshift, min_timeshift, n_kinds, forecast=False):
+        """tsfx_roll_staged: the staged series become their rolled windows (max_timeshift 0: None); forecast: each
+        without its last row, the empty ones dropped (TSFX_FLAG_FORECAST).  Returns (number of union windows, longest
+        window of every kind).  Synchronises the context's stream once."""
         n_rows = ctypes.c_int64(0)
         max_len = np.zeros(n_kinds, dtype=np.int32)
         rc = self.lib.tsfx_roll_staged(self.h, int(rolling_direction), int(max_timeshift), int(min_timeshift),
-                                       ctypes.byref(n_rows), _ptr(max_len), 0)
+                                       ctypes.byref(n_rows), _ptr(max_len), FLAG_FORECAST if forecast else 0)
         self.check(rc, "tsfx_roll_staged")
         return n_rows.value, max_len
 
@@ -248,6 +254,11 @@ class Context:
         """tsfx_staged_row_keys: the naming sort keys of the staged windows, or the package numbers of the staged
         packages, into device memory (8 bytes each)"""
         self.check(self.lib.tsfx_staged_row_keys(self.h, ctypes.c_void_p(keys_ptr)), "tsfx_staged_row_keys")
+
+    def staged_targets(self, rows_ptr):
+        """tsfx_staged_targets: the target input row of every staged forecasting window (-1: none), into device memory
+        (int64)"""
+        self.check(self.lib.tsfx_staged_targets(self.h, ctypes.c_void_p(rows_ptr)), "tsfx_staged_targets")
 
     def extract_staged(self, device_plans, ids_ptr, out_ptr, ld, flags=0):
         """tsfx_extract_staged: device_plans[k] is kind k's DevicePlan (None for a kind without rows)"""

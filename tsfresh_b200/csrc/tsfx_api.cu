@@ -1455,14 +1455,16 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
     S.n_union = 0;
     S.d_times = nullptr;
     S.d_keys = nullptr;
+    S.d_src = nullptr;
     S.has_keys = false;
     S.rolled = false;
     S.packaged = false;
+    S.forecast = false;
     if (n_rows > 0) {
         std::string msg;
         int rc = stacked_stage(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values, kind_codes,
                                kind_code_is_i64, n_kinds, row_time_ns, n_rows, (flags & TSFX_FLAG_KEEP_SORT_KEYS) != 0,
-                               ctx->stream, &msg);
+                               (flags & TSFX_FLAG_KEEP_ROW_NUMBERS) != 0, ctx->stream, &msg);
         if (rc) return fail(ctx, rc, msg);
         CK(cudaStreamSynchronize(ctx->stream));
         const StackedInfo& I = *S.h_info;
@@ -1544,8 +1546,8 @@ extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans,
 
 extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                                 int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags) {
-    (void)flags;
     if (!ctx) return TSFX_E_INVALID;
+    const bool forecast = (flags & TSFX_FLAG_FORECAST) != 0;
     StackedWorkspace& S = ctx->stacked;
     ctx->launches = 0;
     ctx->n_kernels = 0;
@@ -1555,10 +1557,12 @@ extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_
         return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: bad arguments");
     if (S.has_keys && !S.d_keys)
         return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: the rows were staged without TSFX_FLAG_KEEP_SORT_KEYS");
+    if (forecast && S.n_union > 0 && !S.d_src)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: TSFX_FLAG_FORECAST needs rows staged with TSFX_FLAG_KEEP_ROW_NUMBERS");
     S.valid = false;
     *n_rows_out = 0;
     for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
-    if (S.n_union == 0) { S.rolled = true; S.valid = true; return TSFX_OK; }
+    if (S.n_union == 0) { S.rolled = true; S.forecast = forecast; S.valid = true; return TSFX_OK; }
     CK(cudaSetDevice(ctx->device));
     const StackedInfo& I = *S.h_info;
     // the shifts are anchored to the longest (kind, id) series; a window never has more rows than its series, and a
@@ -1572,7 +1576,8 @@ extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_
     const int64_t series = I.kind_series[S.n_kinds];
     const int64_t bound = std::min(rows, series > rows / shifts ? rows : series * shifts);
     std::string msg;
-    int rc = stacked_roll(S, ctx->csr, rolling_direction, max_timeshift, min_timeshift, Lmax, bound, ctx->stream, &msg);
+    int rc = stacked_roll(S, ctx->csr, rolling_direction, max_timeshift, min_timeshift, Lmax, bound, forecast, ctx->stream,
+                          &msg);
     if (rc) return fail(ctx, rc, msg);
     CK(cudaStreamSynchronize(ctx->stream));
     if (I.dup_names)
@@ -1631,6 +1636,18 @@ extern "C" int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys) {
     if (!out_keys) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: NULL out_keys");
     CK(cudaSetDevice(ctx->device));
     CK(cudaMemcpyAsync(out_keys, S.d_ukey, (size_t)S.n_union * 8, cudaMemcpyDeviceToDevice, ctx->stream));
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_staged_targets(tsfx_ctx* ctx, int64_t* out_rows) {
+    if (!ctx) return TSFX_E_INVALID;
+    StackedWorkspace& S = ctx->stacked;
+    if (!S.rolled || !S.forecast)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_staged_targets: no forecasting windows staged (tsfx_roll_staged, TSFX_FLAG_FORECAST)");
+    if (S.n_union == 0) return TSFX_OK;
+    if (!out_rows) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_targets: NULL out_rows");
+    CK(cudaSetDevice(ctx->device));
+    CK(cudaMemcpyAsync(out_rows, S.d_utarget, (size_t)S.n_union * 8, cudaMemcpyDeviceToDevice, ctx->stream));
     return TSFX_OK;
 }
 

@@ -287,7 +287,9 @@ enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T
        // flags, union windows' names
        R_OFF, R_BEGIN, R_LEN, R_ROW, R_ID, R_KEY, R_SCAN, R_UID, R_UKEY,
        // stacked_sub: begin / len / union row of every package in union order inside its kind
-       P_BEGIN, P_LEN, P_ROW, T_SLOTS };
+       P_BEGIN, P_LEN, P_ROW,
+       // input row number of every staged row; stacked_roll with forecast: target row of every window and union window
+       T_SRC, R_TGT, R_UTGT, T_SLOTS };
 static_assert(T_SLOTS <= 32, "StackedWorkspace::bufs");
 
 cudaError_t StackedWorkspace::reserve(int slot, size_t bytes) {
@@ -310,8 +312,8 @@ void StackedWorkspace::release() {
     if (h_info) cudaFreeHost(h_info);
     h_info = nullptr; d_info = nullptr;
     d_values = nullptr; d_times = nullptr; d_begin = nullptr; d_len = nullptr; d_row = nullptr; d_uid = nullptr;
-    d_keys = nullptr; d_ukey = nullptr;
-    valid = false; rolled = false; packaged = false;
+    d_keys = nullptr; d_ukey = nullptr; d_src = nullptr; d_utarget = nullptr;
+    valid = false; rolled = false; packaged = false; forecast = false;
 }
 
 #define STACK_TILE 4096          // rows per CTA of the counting sort
@@ -346,15 +348,16 @@ __global__ void __launch_bounds__(STACK_THREADS) k_stack_count(const uint32_t* _
 
 // Stable scatter of the counting sort: each tile walks its rows in order, 256 at a time; a row's destination is its
 // kind's running base in this tile + the rows of that kind in earlier warps of the step + its rank among its warp's
-// rows of the same kind (__match_any_sync).  Gathers the value (already in CSR order), the union row, the time and the
-// sort key (the last two when asked for).
+// rows of the same kind (__match_any_sync).  Gathers the value (already in CSR order), the union row, the time, the
+// sort key and the input row number (the last three when asked for).
 __global__ void __launch_bounds__(STACK_THREADS) k_stack_scatter(const uint8_t* __restrict__ code, const int* __restrict__ offs,
                                                                  int n_kinds, int64_t n, const float* __restrict__ vals,
                                                                  const int32_t* __restrict__ urow, const int64_t* __restrict__ times,
                                                                  const uint64_t* __restrict__ keys,
                                                                  const uint32_t* __restrict__ perm, const StackedInfo* info,
                                                                  float* __restrict__ out_vals, int32_t* __restrict__ out_row,
-                                                                 int64_t* __restrict__ out_times, uint64_t* __restrict__ out_keys) {
+                                                                 int64_t* __restrict__ out_times, uint64_t* __restrict__ out_keys,
+                                                                 uint32_t* __restrict__ out_src) {
     constexpr int W = STACK_THREADS / 32;
     __shared__ int64_t base[TSFX_MAX_KINDS];
     __shared__ int cnt[W][TSFX_MAX_KINDS];
@@ -378,6 +381,7 @@ __global__ void __launch_bounds__(STACK_THREADS) k_stack_scatter(const uint8_t* 
             out_row[dst] = urow[i];
             if (times) out_times[dst] = times[perm[i]];
             if (keys) out_keys[dst] = keys[perm[i]];
+            if (out_src) out_src[dst] = perm[i];
         }
         __syncthreads();
         for (int kk = threadIdx.x; kk < n_kinds; kk += blockDim.x) {
@@ -467,10 +471,11 @@ __global__ void k_stack_finish(const CsrInfo* csr, StackedInfo* info) {
 
 int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
                   const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
-                  int64_t n, bool keep_keys, cudaStream_t st, std::string* msg) {
+                  int64_t n, bool keep_keys, bool keep_rows, cudaStream_t st, std::string* msg) {
     S.valid = false;
     S.rolled = false;
     S.packaged = false;
+    S.forecast = false;
     S.n_kinds = n_kinds;
     S.has_keys = d_keys != nullptr;
     S.keys_f64 = d_keys && keys_f64;
@@ -495,6 +500,7 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     if (d_times) CKE(S.reserve(T_TIMES, (size_t)n_pad * 8), "alloc times");
     keep_keys = keep_keys && d_keys;
     if (keep_keys) CKE(S.reserve(T_KEYS, (size_t)n_pad * 8), "alloc keys");
+    if (keep_rows) CKE(S.reserve(T_SRC, (size_t)n_pad * 4), "alloc row numbers");
     uint8_t* code = (uint8_t*)S.bufs[T_CODE];
     int32_t* urow = (int32_t*)S.bufs[T_UROW];      // union row of every CSR row; later the series index of every staged row
     int* counts = (int*)S.bufs[T_COUNTS];
@@ -502,6 +508,7 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     S.d_values = (float*)S.bufs[T_VALS];
     S.d_times = d_times ? (int64_t*)S.bufs[T_TIMES] : nullptr;
     S.d_keys = keep_keys ? (uint64_t*)S.bufs[T_KEYS] : nullptr;
+    S.d_src = keep_rows ? (uint32_t*)S.bufs[T_SRC] : nullptr;
     S.d_begin = (int64_t*)S.bufs[T_BEGIN];
     S.d_len = (int32_t*)S.bufs[T_LEN];
     S.d_row = (int32_t*)S.bufs[T_ROW];
@@ -525,7 +532,7 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     k_stack_kind_rows<<<1, 1, 0, st>>>(counts, n_kinds, n_tiles, S.d_info);
     k_stack_scatter<<<n_tiles, STACK_THREADS, 0, st>>>(code, counts, n_kinds, n, W.d_values, urow, d_times,
                                                        keep_keys ? d_keys : nullptr, W.d_perm, S.d_info, S.d_values, srow,
-                                                       S.d_times, S.d_keys);
+                                                       S.d_times, S.d_keys, S.d_src);
     CKE(cudaGetLastError(), "kind scatter kernel");
     CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb3, series_start, urow, (int)(n_pad + 1), st), "series index");
     k_stack_series<<<grid_for(n_pad, 256), 256, 0, st>>>(urow, start, n_pad, S.d_begin, S.d_row);
@@ -555,7 +562,9 @@ __device__ __forceinline__ uint64_t window_name(const uint64_t* __restrict__ key
 }
 
 // windows of every series into cnt[s]; each kind's longest window into info->kind_max_len (zeroed by the caller).  The
-// window lengths are monotone in the shift, so a series' longest window is its first or its last.
+// window lengths are monotone in the shift, so a series' longest window is its first or its last.  Forecast: every window
+// loses its last row.
+template <bool Forecast>
 __global__ void k_roll_count(const int32_t* __restrict__ len, int64_t n_series, RollSpec R, int n_kinds,
                              int32_t* __restrict__ cnt, StackedInfo* info) {
     __shared__ int mx[TSFX_MAX_KINDS];
@@ -571,22 +580,38 @@ __global__ void k_roll_count(const int32_t* __restrict__ len, int64_t n_series, 
         if (n > 0) {
             const int32_t first = roll_window(R, L, t0, &lo);
             const int32_t last = roll_window(R, L, (int32_t)(t0 + (n - 1) * R.amount), &lo);
-            atomicMax(&mx[kind_of_series(info, n_kinds, s)], max(first, last));
+            atomicMax(&mx[kind_of_series(info, n_kinds, s)], max(first, last) - (int32_t)Forecast);
         }
     }
     __syncthreads();
     for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
 }
 
+// 1 when shift u, outside the run of kept shifts, is a window of the roll with min_timeshift given_min_ts and is named
+// `name` too
+__device__ __forceinline__ int dropped_twin(const RollSpec& R, int32_t L, int64_t u, int32_t given_min_ts,
+                                           const uint64_t* __restrict__ keys, int keys_f64, int64_t b, uint64_t name) {
+    if (u < R.first || u > L) return 0;
+    int32_t lo;
+    if (roll_window(R, L, (int32_t)u, &lo) < given_min_ts + 1) return 0;
+    return name == window_name(keys, keys_f64, b, (int32_t)(u - 1));
+}
+
 // One warp per series, one lane per window: the window's view on the staged values, its parent id and its name.  Two
 // windows of one series with the same name (sort keys tied at their naming rows) set info->dup_names.  The slots
 // [off[n_series], bound) get the name that sorts after every real one (id INT64_MAX, key 0x7fff...f: the largest
-// int64, or a NaN above every float64 key).
+// int64, or a NaN above every float64 key).  Forecast: the view loses its last row, and the window's target is the input
+// row number src[] of its naming row, -1 for input row 0.  The reference rolls with the caller's min_timeshift (given_min_ts)
+// and only then drops the last rows, so it also names the one-row windows that R.min_ts >= 1 leaves out here (the shift
+// before the first kept one, or after the last), and merges such a window with a kept neighbour of the same name: that
+// name is flagged too.
+template <bool Forecast>
 __global__ void k_roll_fill(const int64_t* __restrict__ begin, const int32_t* __restrict__ len, const int32_t* __restrict__ row,
                             const int64_t* __restrict__ uid, const uint64_t* __restrict__ keys, int keys_f64,
                             const int32_t* __restrict__ off, int64_t n_series, int64_t bound, RollSpec R,
                             int64_t* __restrict__ wbegin, int32_t* __restrict__ wlen, int64_t* __restrict__ wid,
-                            uint64_t* __restrict__ wkey, StackedInfo* info) {
+                            uint64_t* __restrict__ wkey, StackedInfo* info, const uint32_t* __restrict__ src,
+                            int64_t* __restrict__ wtarget, int32_t given_min_ts) {
     const int lane = threadIdx.x & 31;
     int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -604,10 +629,18 @@ __global__ void k_roll_fill(const int64_t* __restrict__ begin, const int32_t* __
             const int32_t wl = roll_window(R, L, t, &lo);
             const uint64_t name = window_name(keys, keys_f64, b, t - 1);
             wbegin[o + j] = b + lo;
-            wlen[o + j] = wl;
+            wlen[o + j] = wl - (int32_t)Forecast;
             wid[o + j] = id;
             wkey[o + j] = name;
+            if (Forecast) {
+                const uint32_t r = src[b + t - 1];
+                wtarget[o + j] = r == 0 ? -1 : (int64_t)r;
+            }
             if (j > 0 && keys) dup |= name == window_name(keys, keys_f64, b, t - R.amount - 1);
+            if (Forecast && keys) {
+                if (j == 0) dup |= dropped_twin(R, L, (int64_t)t - R.amount, given_min_ts, keys, keys_f64, b, name);
+                if (j == n - 1) dup |= dropped_twin(R, L, (int64_t)t + R.amount, given_min_ts, keys, keys_f64, b, name);
+            }
         }
     }
     if (__any_sync(0xffffffffu, dup) && lane == 0) atomicOr(&info->dup_names, 1);
@@ -632,10 +665,13 @@ struct NameChange {
     }
 };
 
-// union row of every window, name of every union row, the union size
+// union row of every window, name of every union row, the union size; Forecast: the target of every union row, from its
+// first window in name order (the lowest kind's)
+template <bool Forecast>
 __global__ void k_roll_union(const uint32_t* __restrict__ perm, const int32_t* __restrict__ scan, const int32_t* __restrict__ n_windows,
                              const int64_t* __restrict__ wid, const uint64_t* __restrict__ wkey, int32_t* __restrict__ wrow,
-                             int64_t* __restrict__ uid, uint64_t* __restrict__ ukey, StackedInfo* info) {
+                             int64_t* __restrict__ uid, uint64_t* __restrict__ ukey, StackedInfo* info,
+                             const int64_t* __restrict__ wtarget, int64_t* __restrict__ utarget) {
     const int64_t nw = *n_windows;
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
@@ -644,7 +680,11 @@ __global__ void k_roll_union(const uint32_t* __restrict__ perm, const int32_t* _
         const uint32_t w = perm[i];
         const int32_t u = scan[i];
         wrow[w] = u;
-        if (i == 0 || u != scan[i - 1]) { uid[u] = wid[w]; ukey[u] = wkey[w]; }
+        if (i == 0 || u != scan[i - 1]) {
+            uid[u] = wid[w];
+            ukey[u] = wkey[w];
+            if (Forecast) utarget[u] = wtarget[w];
+        }
     }
 }
 
@@ -654,9 +694,11 @@ __global__ void k_roll_kinds(const int32_t* __restrict__ off, int n_kinds, Stack
 }
 
 int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
-                 int32_t Lmax, int64_t bound, cudaStream_t st, std::string* msg) {
+                 int32_t Lmax, int64_t bound, bool forecast, cudaStream_t st, std::string* msg) {
     const int n_kinds = S.n_kinds;
     const int64_t ns = S.h_info->kind_series[n_kinds];
+    const int32_t given_min_ts = min_timeshift;
+    if (forecast) min_timeshift = std::max(min_timeshift, 1);     // a window of one row is empty without its last row
     const RollSpec R = roll_spec(rolling_direction, max_timeshift, min_timeshift, Lmax);
     const size_t nb = (size_t)std::max<int64_t>(bound, 1);
     CKE(S.reserve(R_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
@@ -668,6 +710,12 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
     CKE(S.reserve(R_SCAN, nb * 4), "alloc windows");
     CKE(S.reserve(R_UID, nb * 8), "alloc windows");
     CKE(S.reserve(R_UKEY, nb * 8), "alloc windows");
+    if (forecast) {
+        CKE(S.reserve(R_TGT, nb * 8), "alloc targets");
+        CKE(S.reserve(R_UTGT, nb * 8), "alloc targets");
+    }
+    int64_t* wtarget = forecast ? (int64_t*)S.bufs[R_TGT] : nullptr;
+    int64_t* utarget = forecast ? (int64_t*)S.bufs[R_UTGT] : nullptr;
     int32_t* off = (int32_t*)S.bufs[R_OFF];
     int64_t* wbegin = (int64_t*)S.bufs[R_BEGIN];
     int32_t* wlen = (int32_t*)S.bufs[R_LEN];
@@ -687,11 +735,13 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
     CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
         "memset info");
     CKE(cudaMemsetAsync(off + ns, 0, 4, st), "memset offsets");
-    k_roll_count<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, R, n_kinds, off, S.d_info);
+    (forecast ? k_roll_count<true> : k_roll_count<false>)<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, R, n_kinds, off,
+                                                                                               S.d_info);
     CKE(cudaGetLastError(), "window count kernel");
     CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb1, off, off, (int)(ns + 1), st), "window offsets");
-    k_roll_fill<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(
-        S.d_begin, S.d_len, S.d_row, S.d_uid, S.d_keys, keys_f64, off, ns, bound, R, wbegin, wlen, wid, wkey, S.d_info);
+    (forecast ? k_roll_fill<true> : k_roll_fill<false>)<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(
+        S.d_begin, S.d_len, S.d_row, S.d_uid, S.d_keys, keys_f64, off, ns, bound, R, wbegin, wlen, wid, wkey, S.d_info,
+        S.d_src, wtarget, given_min_ts);
     CKE(cudaGetLastError(), "window fill kernel");
     // the union of the names: sort (id, name), flag and scan the distinct pairs
     if (int rc = sort_rows(W, wid, wkey, keys_f64, bound, st, msg, &perm)) return rc;
@@ -700,13 +750,16 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
         "union rows");
     S.d_uid = (int64_t*)S.bufs[R_UID];
     S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
-    k_roll_union<<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, wid, wkey, wrow, S.d_uid, S.d_ukey, S.d_info);
+    (forecast ? k_roll_union<true> : k_roll_union<false>)<<<grid_for(bound, 256), 256, 0, st>>>(
+        perm, scan, off + ns, wid, wkey, wrow, S.d_uid, S.d_ukey, S.d_info, wtarget, utarget);
     k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
     CKE(cudaGetLastError(), "union kernels");
     S.d_begin = wbegin;
     S.d_len = wlen;
     S.d_row = wrow;
+    S.d_utarget = utarget;
     S.rolled = true;
+    S.forecast = forecast;
     CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
     return TSFX_OK;
 }
@@ -833,8 +886,8 @@ int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, 
         "union rows");
     S.d_uid = (int64_t*)S.bufs[R_UID];
     S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
-    k_roll_union<<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, pid, (const uint64_t*)pnum, prow, S.d_uid,
-                                                       S.d_ukey, S.d_info);
+    k_roll_union<false><<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, pid, (const uint64_t*)pnum, prow, S.d_uid,
+                                                              S.d_ukey, S.d_info, nullptr, nullptr);
     k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
     CKE(cudaGetLastError(), "union kernels");
     // The packages were filled series by series, (parent id, package number) order inside a kind, but the union rows

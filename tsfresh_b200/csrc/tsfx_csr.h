@@ -114,6 +114,8 @@ struct StackedWorkspace {
     uint64_t* d_keys = nullptr;   // sort keys (raw bits) in the order of d_values (stacked_stage with keep_keys)
     uint64_t* d_ukey = nullptr;   // after stacked_roll: naming sort key of every union window (raw bits); after
                                   // stacked_sub: package number of every union package (int64)
+    uint32_t* d_src = nullptr;    // input row number of every staged row (stacked_stage with keep_rows)
+    int64_t* d_utarget = nullptr; // after stacked_roll with forecast: target row of every union window (-1: none)
     StackedInfo* h_info = nullptr;   // pinned
     StackedInfo* d_info = nullptr;
     int n_kinds = 0;
@@ -123,6 +125,7 @@ struct StackedWorkspace {
     bool keys_f64 = false;        //   float64 ones
     bool rolled = false;          // the staged series have been turned into windows (stacked_roll)
     bool packaged = false;        // the staged series have been cut into packages (stacked_sub)
+    bool forecast = false;        // the windows are make_forecasting_frame's (stacked_roll with forecast)
     void* bufs[32] = {nullptr};
     size_t caps[32] = {0};
     cudaError_t reserve(int slot, size_t bytes);
@@ -133,10 +136,11 @@ struct StackedWorkspace {
 // Stages n_rows device rows (ids, sort keys (nullptr: input order), float32 values, kind codes (int32 / int64; nullptr:
 // every row is kind 0), optional int64 row times) into S, then copies S.d_info to S.h_info.  Asynchronous: the caller
 // synchronises and checks the flags before it relies on the sizes.  Uses W's sort buffers as scratch.  keep_keys: the
-// sort keys follow the rows into S.d_keys (stacked_roll names its windows by them).
+// sort keys follow the rows into S.d_keys (stacked_roll names its windows by them).  keep_rows: every staged row's input
+// row number goes to S.d_src (stacked_roll with forecast finds the targets by them).
 int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
                   const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
-                  int64_t n_rows, bool keep_keys, cudaStream_t st, std::string* msg);
+                  int64_t n_rows, bool keep_keys, bool keep_rows, cudaStream_t st, std::string* msg);
 
 // Rolled windows (roll_time_series, tsfx_roll.cuh) of the staged series, as new staged series: every window is a view
 // (d_begin, d_len) on the unchanged d_values, so each kind keeps its aligned rows.  Per series a count of its windows, a
@@ -145,8 +149,12 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
 // d_row of every window, d_uid / d_ukey of every union row.  d_info gets the window ranges of the kinds (kind_series),
 // their longest windows (kind_max_len), n_union and dup_names, and is copied to h_info (the caller synchronises).
 // Lmax = the longest staged series (the shifts' anchor); bound >= the number of windows.
+// forecast (make_forecasting_frame, needs S.d_src): only windows of at least max(min_timeshift, 1) + 1 rows are kept,
+// every one of them loses its last row (so none is empty), and its target is the input row number of its naming row (-1
+// for input row 0, which the reference's y = x[1:] leaves out); the first window of every union row passes its target on
+// to d_utarget.  A name shared with a one-row window that min_timeshift keeps but the drop empties sets dup_names too.
 int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
-                 int32_t Lmax, int64_t bound, cudaStream_t st, std::string* msg);
+                 int32_t Lmax, int64_t bound, bool forecast, cudaStream_t st, std::string* msg);
 
 // Fixed-length packages (add_sub_time_series_index) of the staged series, as new staged series: package j of a series
 // of n rows is the view on its rows [j * L, min((j + 1) * L, n)), so each kind keeps its aligned rows.  Same structure as

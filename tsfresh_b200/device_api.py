@@ -28,6 +28,12 @@ synchronisation to learn the number of windows.
 
 is extract_features(add_sub_time_series_index(frame, 1000, ...), column_id="id") for the same rows: tsfx_sub_staged
 cuts the staged series into consecutive packages of sub_length rows (views again), named (package number, parent id).
+
+    X, window_keys, y, columns = extract_features_forecasting_device(x, "sensor", max_timeshift=255, rolling_direction=1)
+
+is make_forecasting_frame(x, ...) extracted, with its target vector aligned to the rows of X: the rolled call on one
+series whose windows tsfx_roll_staged (TSFX_FLAG_FORECAST) shortens by their last row, and whose targets it reports as
+input row numbers that torch gathers from x.
 """
 import numbers
 
@@ -243,8 +249,8 @@ def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=Non
     columns.  Runs on torch's current stream and blocks the host once, to learn the number of ids.  Raises ValueError for
     NaN values or sort keys, kind codes out of range and series longer than their kind's plan allows, before any feature
     kernel runs."""
-    X, row_ids, _, columns = _extract_staged(ids, values, sort, kind, kinds, times, None, default_fc_parameters,
-                                             kind_to_fc_parameters, impute_function)
+    X, row_ids, _, columns, _ = _extract_staged(ids, values, sort, kind, kinds, times, None, default_fc_parameters,
+                                                kind_to_fc_parameters, impute_function)
     return X, row_ids, columns
 
 
@@ -287,7 +293,63 @@ def extract_features_rolled_device(ids, values, sort=None, kind=None, *, kinds=N
     longer than their kind's plan allows, before any feature kernel runs."""
     roll = _roll_args(rolling_direction, max_timeshift, min_timeshift)
     return _extract_staged(ids, values, sort, kind, kinds, None, roll, default_fc_parameters, kind_to_fc_parameters,
-                           impute_function)
+                           impute_function)[:4]
+
+
+def extract_features_forecasting_device(x, kind, max_timeshift, rolling_direction, min_timeshift=0, *, index=None,
+                                        default_fc_parameters=None, kind_to_fc_parameters=None, impute_function=None):
+    """Extracts features from the forecasting windows of one series held in a CUDA tensor, with their targets.
+
+    x: 1-D CUDA tensor, float32, float64, float16 or bfloat16 (rounded to float32 for the features).  index: 1-D CUDA
+    tensor of int64 or float64 sort keys, the role of a pd.Series' index (None: 0 .. n-1; datetimes as int64
+    nanoseconds).  kind, max_timeshift, rolling_direction and min_timeshift: as make_forecasting_frame.
+    default_fc_parameters, kind_to_fc_parameters and impute_function: as extract_features_long_device.
+
+    Returns (X, window_keys, y, columns).  X and columns are what extract_features(df_shift, column_id="id",
+    column_sort="time", column_kind="kind", column_value="value") returns for (df_shift, _) = make_forecasting_frame(...)
+    on the equivalent Series: the series is rolled as roll_time_series rolls it, every window loses its last row and the
+    windows this empties are dropped.  Row r of X is the window named ("id", window_keys[r]), names ascending;
+    window_keys has the index's dtype (int64 row numbers without an index).  y (x's dtype, bit-exact) is the target of
+    every row: x at the row that names the window (its last row before the drop for a positive direction, its first row
+    for a negative one), what make_forecasting_frame's y holds for that name.  One window has no target: the one named by
+    x[0], which make_forecasting_frame's y (x[1:]) leaves out.  With a positive direction and an ascending index it is
+    the one-row window that the drop empties; with a negative direction (or an index whose first key is not its smallest)
+    it is a row of X, and its y is NaN.  Drop the rows where y is NaN before select_features_device.
+
+    Runs on torch's current stream and blocks the host twice: to stage the rows and to count the windows.  Raises
+    roll_time_series's errors for its arguments, and for a series of zero or one rows, before the device is touched, and
+    ValueError for NaN values or index keys, two windows with the same name (index keys tied at their naming rows,
+    counting the one-row windows that the drop of the last row empties, which the reference merges too) and windows
+    longer than the plan allows, before any feature kernel runs.  The plan's length limits apply to the windows, not to
+    the series."""
+    import torch
+    roll = _roll_args(rolling_direction, max_timeshift, min_timeshift)
+    for name, t in (("x", x), ("index", index)):
+        if t is None and name == "index":
+            continue
+        if not isinstance(t, torch.Tensor):
+            raise TypeError("%s must be a torch.Tensor, not %s" % (name, type(t).__name__))
+        if t.ndim != 1:
+            raise ValueError("%s must be 1-D, got shape %s" % (name, tuple(t.shape)))
+    if index is not None and index.shape[0] != x.shape[0]:
+        raise ValueError("index has %d entries, x %d" % (index.shape[0], x.shape[0]))
+    if x.dtype not in (torch.float32, torch.float64, torch.float16, torch.bfloat16):
+        raise TypeError("x must be float32, float64, float16 or bfloat16, not %s" % x.dtype)
+    if index is not None and index.dtype not in (torch.int64, torch.float64):
+        raise TypeError("index must be int64 or float64, not %s" % index.dtype)
+    if x.shape[0] <= 1:
+        raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
+    _check_colname(kind)
+    if x.device.type != "cuda":
+        raise ValueError("x must be a CUDA tensor, got one on %s" % x.device)
+    if index is not None and index.device != x.device:
+        raise ValueError("index is on %s, x on %s" % (index.device, x.device))
+    X, _, window_keys, columns, targets = _extract_staged(None, x, index, None, [kind], None, roll, default_fc_parameters,
+                                                          kind_to_fc_parameters, impute_function, forecast=True)
+    with torch.cuda.device(x.device):
+        nan = torch.full((), float("nan"), dtype=x.dtype, device=x.device)
+        y = torch.where(targets >= 0, x[targets.clamp(min=0)], nan)
+    return X, window_keys, y, columns
 
 
 def _sub_length(sub_length):
@@ -323,20 +385,21 @@ def extract_features_sub_device(ids, values, sort=None, kind=None, *, kinds=None
     NaN values or sort keys, kind codes out of range and packages longer than their kind's plan allows, before any
     feature kernel runs."""
     L = _sub_length(sub_length)
-    X, package_ids, package_numbers, columns = _extract_staged(ids, values, sort, kind, kinds, times, None,
-                                                               default_fc_parameters, kind_to_fc_parameters,
-                                                               impute_function, sub_length=L)
+    X, package_ids, package_numbers, columns, _ = _extract_staged(ids, values, sort, kind, kinds, times, None,
+                                                                  default_fc_parameters, kind_to_fc_parameters,
+                                                                  impute_function, sub_length=L)
     return X, package_numbers, package_ids if ids is not None else None, columns
 
 
 def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_parameters, kind_to_fc_parameters,
-                    impute_function, sub_length=None):
-    """(X, row ids, row keys, columns) of long-format rows, staged by kind and extracted; with roll = (direction,
-    max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows' naming keys),
-    with sub_length they are cut into packages first (row keys: the package numbers; ids may then be None), else row
-    keys is None."""
+                    impute_function, sub_length=None, forecast=False):
+    """(X, row ids, row keys, columns, targets) of long-format rows, staged by kind and extracted; with roll =
+    (direction, max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows'
+    naming keys), with sub_length they are cut into packages first (row keys: the package numbers; ids may then be
+    None), else row keys is None.  forecast (with roll; ids may then be None): the windows are make_forecasting_frame's
+    and targets holds the target input row of every window (-1: none), else targets is None."""
     import torch
-    n, kinds = _long_layout(ids, values, sort, kind, kinds, times, need_ids=sub_length is None)
+    n, kinds = _long_layout(ids, values, sort, kind, kinds, times, need_ids=sub_length is None and not forecast)
     if roll is not None and n <= 1:
         raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
     default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
@@ -349,7 +412,7 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
         if t is not None and t.device != dev:
             raise ValueError("%s is on %s, values on %s" % (name, t.device, dev))
     mode = _lib.IMPUTE_RANGE if impute_function is impute else _lib.IMPUTE_ZERO if impute_function is impute_dataframe_zero else None
-    row_keys = None
+    row_keys = targets = None
     with torch.cuda.device(dev):
         v = values.contiguous() if values.dtype == torch.float32 else values.to(torch.float32).contiguous()
         i = torch.zeros(n, dtype=torch.int64, device=dev) if ids is None else ids.contiguous()
@@ -364,11 +427,14 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
                 n_rows, rows, _ = ctx.stage_long_stacked(
                     i.data_ptr(), 0 if s is None else s.data_ptr(), s is not None and s.dtype == torch.float64,
                     v.data_ptr(), 0 if k is None else k.data_ptr(), k is not None and k.dtype == torch.int64, len(kinds),
-                    0 if t is None else t.data_ptr(), n, keep_sort_keys=roll is not None)
+                    0 if t is None else t.data_ptr(), n, keep_sort_keys=roll is not None, keep_row_numbers=forecast)
                 if roll is not None:
-                    n_rows, _ = ctx.roll_staged(*roll, len(kinds))
+                    n_rows, _ = ctx.roll_staged(*roll, len(kinds), forecast=forecast)
                     row_keys = torch.empty(n_rows, dtype=torch.int64 if s is None else s.dtype, device=dev)
                     ctx.staged_row_keys(row_keys.data_ptr())
+                    if forecast:
+                        targets = torch.empty(n_rows, dtype=torch.int64, device=dev)
+                        ctx.staged_targets(targets.data_ptr())
                 elif sub_length is not None:
                     n_rows, _ = ctx.sub_staged(sub_length, len(kinds))
                     row_keys = torch.empty(n_rows, dtype=torch.int64, device=dev)
@@ -389,4 +455,4 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
         df = pd.DataFrame(X.cpu().numpy(), columns=columns)
         impute_function(df)
         X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
-    return X, row_ids, row_keys, columns
+    return X, row_ids, row_keys, columns, targets

@@ -378,7 +378,7 @@ def extract_features(timeseries_container, default_fc_parameters=None, kind_to_f
     default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
     from .rolling import RolledTimeSeries
     if isinstance(timeseries_container, RolledTimeSeries):
-        return _extract_rolled(timeseries_container, default_fc_parameters, kind_to_fc_parameters, impute_function,
+        return _extract_rolled(timeseries_container._for_columns(column_kind, column_value), default_fc_parameters, kind_to_fc_parameters, impute_function,
                                show_warnings, device)
     if distributor is not None:
         from .distributor import is_distributor

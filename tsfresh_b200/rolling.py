@@ -12,6 +12,10 @@ include/tsfx.h); the result is a `RolledTimeSeries` that `tsfresh_b200.extract_f
 Same arguments, validation errors and window ids as the reference; `chunksize / n_jobs / distributor / progress bar`
 are accepted for signature compatibility only.  `rolled.to_frame()` materialises the reference's DataFrame
 (testing / interchange; not used by the extraction path).
+
+make_forecasting_frame (dataframe_functions.py:606-680) rolls one series the same way and shortens every window by its
+last row; its df_shift is a ForecastingFrame of such views, and extract_features reads it as the reference reads its
+frame with column_id="id", column_sort="time" and column_value="value" (and column_kind="kind").
 """
 import warnings
 
@@ -66,6 +70,65 @@ class RolledTimeSeries:
         for k, v in self.values.items():
             out[k] = v[rows]
         return pd.DataFrame(out)
+
+    def _for_columns(self, column_kind, column_value):
+        """the windows as extract_features(self, column_kind=..., column_value=...) reads them: a rolled frame names its
+        kinds itself"""
+        return self
+
+
+class ForecastingFrame(RolledTimeSeries):
+    """make_forecasting_frame's df_shift: windows of one series without their last rows, as views on its values (x's
+    dtype, time order); to_frame() gives the reference's columns time, value, kind and id, in its order."""
+
+    def __init__(self, values, begin, length, ids, parent, id_row, sort_values, kind):
+        super().__init__({"value": values}, begin, length, ids, parent, id_row, sort_values, "time")
+        self.kind = kind
+
+    def to_frame(self):
+        out = super().to_frame()
+        out["kind"] = [self.kind] * len(out)
+        return out[["time", "value", "kind", "id"]]
+
+    def _for_columns(self, column_kind, column_value):
+        # the frame's value column is "value"; with column_kind its one kind is named by the kind column
+        name = str(self.kind) if column_kind is not None else "value"
+        return RolledTimeSeries({name: self.values["value"]}, self.begin, self.length, self.ids, self.parent, self.id_row,
+                                self.sort_values, self.column_sort)
+
+
+def make_forecasting_frame(x, kind, max_timeshift, rolling_direction, min_timeshift=0):
+    """dataframe_functions.py:606-680: (df_shift, y) for one series x (list, numpy array or pd.Series, whose index is
+    then the time).  df_shift holds roll_time_series's windows of x, each without its last row and the windows this
+    empties left out, as a ForecastingFrame; y (named "value", x's dtype) is x[1:] indexed by ("id", time), restricted
+    to the names of the windows, in x's order.  Raises ValueError when two windows have the same name (the index ties at
+    the rows that name them), which the reference merges into one series."""
+    n = len(x)
+    t = x.index if isinstance(x, pd.Series) else range(n)
+    df = pd.DataFrame({"id": ["id"] * n, "time": t, "value": x, "kind": kind})
+    if rolling_direction == 0:
+        raise ValueError("Rolling direction of 0 is not possible")
+    if max_timeshift is not None and max_timeshift <= 0:
+        raise ValueError("max_timeshift needs to be positive!")
+    if min_timeshift < 0:
+        raise ValueError("min_timeshift needs to be positive or zero!")
+    if n <= 1:
+        raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
+    if df["time"].isnull().any():
+        raise ValueError("You have NaN values in your sort column.")
+    order = np.argsort(df["time"].to_numpy(), kind="stable")       # the series order _roll_frame would choose
+    rolled = _roll_frame(df[["id", "time", "value"]].iloc[order], "id", "time", rolling_direction, max_timeshift,
+                         min_timeshift, False, None)
+    if len(set(rolled.ids)) != len(rolled.ids):
+        # the reference merges windows of one name into one series before it drops a row of it: not a view
+        raise ValueError("two windows have the same name (id, time): the index ties at the rows that name them")
+    keep = np.flatnonzero(rolled.length >= 2)                       # a window of one row is empty without its last row
+    ids = [rolled.ids[i] for i in keep]
+    df_shift = ForecastingFrame(df["value"].to_numpy()[order], rolled.begin[keep], rolled.length[keep] - 1, ids,
+                                rolled.parent[keep], rolled.id_row[keep], rolled.sort_values, kind)
+    y = df["value"][1:]
+    y.index = map(lambda v: ("id", v), y.index)
+    return df_shift, y[y.index.isin(set(ids))]
 
 
 def roll_time_series(df_or_dict, column_id, column_sort=None, column_kind=None, rolling_direction=1, max_timeshift=None,
