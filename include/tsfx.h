@@ -67,6 +67,9 @@ extern "C" {
 #define TSFX_FLAG_KEEP_ROW_NUMBERS 128u /* tsfx_stage_long_stacked: keep every staged row's input row number (4 bytes per row),
                                   * which tsfx_roll_staged with TSFX_FLAG_FORECAST finds the targets by */
 #define TSFX_FLAG_FORECAST 256u  /* tsfx_roll_staged: make_forecasting_frame's windows (see tsfx_staged_targets) */
+#define TSFX_FLAG_DEFER_CHECK 512u /* with TSFX_FLAG_DEVICE_PTRS, tsfx_extract_csr / tsfx_extract_dense validate the input on
+                                  * the device and report to the status buffer of tsfx_set_status instead of returning an
+                                  * error; see "Deferred input check" below */
 
 /* tsfx_impute modes (tsfresh/utilities/dataframe_functions.py) */
 #define TSFX_IMPUTE_RANGE 0      /* impute :49-78: +inf -> max, -inf -> min, NaN -> median of the finite values */
@@ -192,7 +195,9 @@ void tsfx_ctx_destroy(tsfx_ctx* ctx);
  * stream the caller is on.  cuda_stream is a stream of the context's device, or NULL for the stream the context was
  * created with; pass cudaStreamLegacy ((void*)1) for the legacy default stream.  The new stream first waits for
  * everything already enqueued on the old one (the calls reuse the context's scratch); the side streams, copy streams
- * and timing events of later calls fork from and join to the new stream.  Does not block the host. */
+ * and timing events of later calls fork from and join to the new stream.  Does not block the host.  When the old or the
+ * new stream is capturing a CUDA graph, the new stream does not wait (an event recorded on one side of a capture cannot
+ * order work on the other): ordering the graph's launches against other work on the context is then the caller's. */
 int tsfx_ctx_set_stream(tsfx_ctx* ctx, void* cuda_stream);
 const char* tsfx_last_error(const tsfx_ctx* ctx); /* ctx may be NULL: last creation error */
 int tsfx_sync(tsfx_ctx* ctx);
@@ -231,6 +236,36 @@ int tsfx_set_out_ld(tsfx_ctx* ctx, int32_t ld);
  * them (tsfx_extract_long carries them through its sort).  A plan with linear_trend_timewise columns and no row times
  * is TSFX_E_INVALID. */
 int tsfx_set_row_times(tsfx_ctx* ctx, const int64_t* row_time_ns, int64_t n_rows, uint32_t flags);
+
+/* Deferred input check, for calls that only enqueue work (no allocation, copy to the host or synchronisation), so that
+ * they overlap other work and can be captured in a CUDA graph:
+ *   tsfx_prepare       does ahead of time every lazy step a device-pointer call of `plan` with at most n_series series of
+ *                      at most max_len samples takes: the length check (TSFX_E_TOO_LONG), the working memory (256 MB, or
+ *                      1 GB for max_len > 1 024, plus the staging matrices and the check's per-series buffers) and the
+ *                      FFT / Ricker tables.  Blocks until the tables are filled.  Prepare every plan a context will run, before
+ *                      capturing any call in a graph: a later, larger tsfx_prepare may move the working memory.
+ *   tsfx_set_status    the caller's device buffer of TSFX_STATUS_WORDS int64 words (zeroed by the caller) that the
+ *                      following TSFX_FLAG_DEFER_CHECK calls report to; NULL removes it.
+ * A TSFX_FLAG_DEFER_CHECK call (needs TSFX_FLAG_DEVICE_PTRS and a prepared shape, and excludes
+ * TSFX_FLAG_CHECK_DEVICE_INPUT and TSFX_FLAG_IMPUTE) makes one pass over its input that rejects a series for a NaN value,
+ * an invalid view (len < 1, begin < 0 or begin + len > n_values) or a view longer than the declared max_len (CSR: the
+ * tsfx_set_max_len_hint value, which is then required; dense: len).  CSR calls hand the groups private views, in which a
+ * rejected view is the one-sample view (0, 1); dense calls hand them the input as it is.  After the groups, every column
+ * of a rejected series is set to NaN in `out` (honouring tsfx_set_out_ld).  The call then counts itself in
+ * status[TSFX_STATUS_CALLS] and, if no earlier call since the caller last zeroed status[TSFX_STATUS_BAD] rejected a
+ * series and this one did, stores the count in status[TSFX_STATUS_BAD] and the call's first series of each reason in the
+ * three reason words (-1: none). */
+#define TSFX_STATUS_CALLS 0
+#define TSFX_STATUS_BAD 1
+#define TSFX_STATUS_VIEW 2       /* first series with an invalid view */
+#define TSFX_STATUS_LONG 3       /* first valid series longer than max_len */
+#define TSFX_STATUS_NAN 4        /* first other series with a NaN value */
+#define TSFX_STATUS_WORDS 8
+int tsfx_prepare(tsfx_ctx* ctx, const tsfx_plan* plan, int64_t n_series, int32_t max_len);
+int tsfx_set_status(tsfx_ctx* ctx, int64_t* status);
+/* Longest series a plan of these columns accepts (TSFX_E_TOO_LONG beyond; 2^31 - 1 when no group limits it), or
+ * TSFX_E_INVALID for an unknown calculator.  Needs no context or device. */
+int32_t tsfx_plan_max_len(const tsfx_feature_desc* descs, int32_t n_descs);
 
 /* Dense fast path: n_series series of identical length `len`, back to back. */
 int tsfx_extract_dense(tsfx_ctx* ctx, const tsfx_plan* plan, const float* values, int64_t n_series,

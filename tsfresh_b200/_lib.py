@@ -21,6 +21,8 @@ FLAG_CHECK_DEVICE_INPUT = 32
 FLAG_KEEP_SORT_KEYS = 64
 FLAG_KEEP_ROW_NUMBERS = 128
 FLAG_FORECAST = 256
+FLAG_DEFER_CHECK = 512
+STATUS_CALLS, STATUS_BAD, STATUS_VIEW, STATUS_LONG, STATUS_NAN, STATUS_WORDS = 0, 1, 2, 3, 4, 8
 STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy default stream for tsfx_ctx_set_stream
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
@@ -41,7 +43,8 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_last_launch_count", "tsfx_last_kernels", "tsfx_kernel_variants", "tsfx_impute", "tsfx_extract_long_alloc", "tsfx_host_alloc", "tsfx_host_free",
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
            "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged",
-           "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged", "tsfx_staged_targets"]
+           "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged", "tsfx_staged_targets",
+           "tsfx_prepare", "tsfx_set_status", "tsfx_plan_max_len"]
 
 
 def load():
@@ -96,6 +99,10 @@ def load():
         lib.tsfx_staged_row_keys.argtypes = [vp, vp]
         lib.tsfx_sub_staged.argtypes = [vp, i64, ctypes.POINTER(i64), vp, u32]
         lib.tsfx_staged_targets.argtypes = [vp, vp]
+        lib.tsfx_prepare.argtypes = [vp, vp, i64, i32]
+        lib.tsfx_set_status.argtypes = [vp, vp]
+        lib.tsfx_plan_max_len.argtypes = [vp, i32]
+        lib.tsfx_plan_max_len.restype = i32
         _lib = lib
         return lib
 
@@ -111,6 +118,15 @@ def kernel_variants():
     names = (ctypes.c_char_p * n)()
     lib.tsfx_kernel_variants(names, n)
     return [names[i].decode() for i in range(n)]
+
+
+def plan_max_len(plan):
+    """Longest series `plan` accepts (tsfx_plan_max_len; 2^31 - 1: no limit).  Needs no device."""
+    descs = np.ascontiguousarray(plan.descs, dtype=DESC_DTYPE)
+    m = load().tsfx_plan_max_len(_ptr(descs), len(descs))
+    if m < 0:
+        raise ValueError("tsfx_plan_max_len: unknown calculator in the plan")
+    return int(m)
 
 
 def _ptr(a):
@@ -170,6 +186,10 @@ class Context:
         """tsfx_ctx_set_stream: enqueue the following calls on `stream` (a cudaStream_t as int; None: the stream the
         context was created with; STREAM_LEGACY: the legacy default stream)."""
         self.check(self.lib.tsfx_ctx_set_stream(self.h, ctypes.c_void_p(stream) if stream else None), "tsfx_ctx_set_stream")
+
+    def set_status(self, status_ptr):
+        """tsfx_set_status: the device int64 words (TSFX_STATUS_WORDS, zeroed) that FLAG_DEFER_CHECK calls report to"""
+        self.check(self.lib.tsfx_set_status(self.h, ctypes.c_void_p(status_ptr or None)), "tsfx_set_status")
 
     def set_out_ld(self, ld):
         """tsfx_set_out_ld: row stride (doubles) of `out` of the following device-pointer calls; 0 = the plan's n_cols"""
@@ -421,19 +441,27 @@ class DevicePlan:
             ctx.check(rc, "tsfx_extract_long")
         return n_series.value
 
+    def prepare(self, n_series, max_len):
+        """tsfx_prepare: makes calls of up to n_series series of up to max_len samples allocation-free.  Blocks."""
+        rc = self.ctx.lib.tsfx_prepare(self.ctx.h, self.h, int(n_series), int(max_len))
+        self.ctx.check(rc, "tsfx_prepare")
+
     # ---- device-pointer entry points (torch tensors own the memory) ----------------------------
     # checked: the checked pass (TSFX_FLAG_CHECK_DEVICE_INPUT) first validates the views, measures the longest one and
-    # scans the values for NaN on the device, before any kernel group runs
-    def extract_dense_device(self, values_ptr, n_series, length, out_ptr, timing=False, checked=False):
-        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0)
+    # scans the values for NaN on the device, before any kernel group runs.  deferred: TSFX_FLAG_DEFER_CHECK (the
+    # context's status buffer gets the verdict; CSR views are held to max_len)
+    def extract_dense_device(self, values_ptr, n_series, length, out_ptr, timing=False, checked=False, deferred=False):
+        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0) \
+            | (FLAG_DEFER_CHECK if deferred else 0)
         rc = self.ctx.lib.tsfx_extract_dense(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_series, length,
                                              ctypes.c_void_p(out_ptr), flags)
         self.ctx.check(rc, "tsfx_extract_dense")
 
     def extract_csr_device(self, values_ptr, n_values, begin_ptr, len_ptr, n_series, out_ptr, timing=False, max_len=0,
-                           checked=False):
+                           checked=False, deferred=False):
         """max_len: upper bound of the series lengths if the caller knows one (keeps an unchecked call asynchronous)"""
-        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0)
+        flags = FLAG_DEVICE_PTRS | (FLAG_TIMING if timing else 0) | (FLAG_CHECK_DEVICE_INPUT if checked else 0) \
+            | (FLAG_DEFER_CHECK if deferred else 0)
         if not checked:
             self.ctx.check(self.ctx.lib.tsfx_set_max_len_hint(self.ctx.h, int(max_len)), "tsfx_set_max_len_hint")
         rc = self.ctx.lib.tsfx_extract_csr(self.ctx.h, self.h, ctypes.c_void_p(values_ptr), n_values,

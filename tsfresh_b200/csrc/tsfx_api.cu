@@ -261,6 +261,12 @@ struct tsfx_ctx {
     int64_t times_rows = -1;
     int max_len_hint = 0;        // tsfx_set_max_len_hint: longest series of the coming device-pointer CSR calls
     int out_ld = 0;              // tsfx_set_out_ld: row stride of `out` of the coming device-pointer calls (0: n_cols)
+    // TSFX_FLAG_DEFER_CHECK: the largest shape tsfx_prepare made ready, the caller's status words (tsfx_set_status) and
+    // the check's buffers: first series per reason, then per series its private view and its reject reason
+    int64_t prep_series = 0;
+    int prep_len = 0;
+    int64_t* status = nullptr;
+    DevBuf defer;
     HostPool pool;
     Stager stager;
     // multi-GPU result placement (tsfx_set_peer_outputs): peers' mapped result matrices
@@ -415,6 +421,7 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     cudaStreamSynchronize(ctx->home_stream);
     ctx->values.release(); ctx->begin.release(); ctx->len.release(); ctx->out.release(); ctx->misc.release(); ctx->stage.release();
     ctx->times.release(); ctx->times_sorted.release(); ctx->kvals.release(); ctx->kvals_sorted.release();
+    ctx->defer.release();
     ctx->csr.release();
     ctx->stacked.release();
     ctx->imp.release();
@@ -438,14 +445,24 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     delete ctx;
 }
 
+// a stream that is capturing a CUDA graph (or whose capture has been invalidated)
+static bool capturing(cudaStream_t s) {
+    cudaStreamCaptureStatus st = cudaStreamCaptureStatusNone;
+    if (cudaStreamIsCapturing(s, &st) != cudaSuccess) { cudaGetLastError(); return true; }
+    return st != cudaStreamCaptureStatusNone;
+}
+
 extern "C" int tsfx_ctx_set_stream(tsfx_ctx* ctx, void* cuda_stream) {
     if (!ctx) return TSFX_E_INVALID;
     cudaStream_t next = cuda_stream ? (cudaStream_t)cuda_stream : ctx->home_stream;
     if (next == ctx->stream) return TSFX_OK;
     CK(cudaSetDevice(ctx->device));
-    // the next calls reuse the scratch (and twiddle / Ricker tables) the work on the old stream may still be using
-    CK(cudaEventRecord(ctx->ev_rebind, ctx->stream));
-    CK(cudaStreamWaitEvent(next, ctx->ev_rebind, 0));
+    // the next calls reuse the scratch (and twiddle / Ricker tables) the work on the old stream may still be using; an
+    // event cannot order work across the boundary of a graph capture, so there the caller orders it
+    if (!capturing(ctx->stream) && !capturing(next)) {
+        CK(cudaEventRecord(ctx->ev_rebind, ctx->stream));
+        CK(cudaStreamWaitEvent(next, ctx->ev_rebind, 0));
+    }
     ctx->stream = next;
     return TSFX_OK;
 }
@@ -752,17 +769,10 @@ static int check_lengths(tsfx_ctx* ctx, const tsfx_plan* P, int max_len) {
     return TSFX_OK;
 }
 
-static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int max_len, double* d_out, uint32_t flags, int ld = 0) {
-    if (ld <= 0) ld = P->ncols;          // row stride of the caller's matrix
-    const bool timing = (flags & TSFX_FLAG_TIMING) != 0;
-    for (int g = 0; g < G_EVENTS; ++g) ctx->ev_used[g] = false;
-    ctx->launches = 0;
-    ctx->n_kernels = 0;
-    if (R.n_series == 0) return TSFX_OK;
-    const int staged = P->cum[G_COUNT];
-    if (staged == 0) return TSFX_OK;
-    if (int rc = check_lengths(ctx, P, max_len)) return rc;      // every group's length limit before any group runs
-    CK(ctx->stage.reserve((size_t)R.n_series * staged * sizeof(double)));
+// the working memory and tables the groups of P need for n_series series of at most max_len samples (tsfx_prepare
+// makes them ready ahead of time)
+static int reserve_groups(tsfx_ctx* ctx, const tsfx_plan* P, int64_t n_series, int max_len) {
+    CK(ctx->stage.reserve((size_t)n_series * P->cum[G_COUNT] * sizeof(double)));
     CK(ctx->misc.reserve(max_len > 1024 ? ((size_t)1 << 30) : ((size_t)256 << 20)));      // global working regions for series too long for shared memory
     if (!P->host[G_SPECTRAL].empty()) {      // FFT twiddle table (filled once, on the main stream, before any fork)
         int p2 = 1;
@@ -780,6 +790,20 @@ static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int
         int rc = ensure_ricker(ctx);
         if (rc) return rc;
     }
+    return TSFX_OK;
+}
+
+static int run_groups(tsfx_ctx* ctx, const tsfx_plan* P, const SeriesRef& R, int max_len, double* d_out, uint32_t flags, int ld = 0) {
+    if (ld <= 0) ld = P->ncols;          // row stride of the caller's matrix
+    const bool timing = (flags & TSFX_FLAG_TIMING) != 0;
+    for (int g = 0; g < G_EVENTS; ++g) ctx->ev_used[g] = false;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (R.n_series == 0) return TSFX_OK;
+    const int staged = P->cum[G_COUNT];
+    if (staged == 0) return TSFX_OK;
+    if (int rc = check_lengths(ctx, P, max_len)) return rc;      // every group's length limit before any group runs
+    if (int rc = reserve_groups(ctx, P, R.n_series, max_len)) return rc;
     // kernel groups are independent (own staging matrix): optionally spread them over side streams
     const int nstreams = timing ? 1 : env_streams();
     if (nstreams > 1) {
@@ -934,6 +958,75 @@ static int check_device_input(tsfx_ctx* ctx, const float* values, int64_t n_valu
     return TSFX_OK;
 }
 
+// TSFX_FLAG_DEFER_CHECK buffers, laid out for ctx->prep_series series
+struct DeferBufs {
+    unsigned long long* first;   // n_series - s of the first rejected series s per reason (0: none)
+    int64_t* vbegin;             // private views (CSR)
+    int32_t* vlen;
+    uint8_t* reject;             // reject reason per series
+};
+static size_t defer_bytes(int64_t n_series) { return 64 + (size_t)n_series * 13; }
+static DeferBufs defer_bufs(tsfx_ctx* ctx) {
+    char* p = (char*)ctx->defer.p;
+    const size_t n = (size_t)ctx->prep_series;
+    return {(unsigned long long*)p, (int64_t*)(p + 64), (int32_t*)(p + 64 + 8 * n), (uint8_t*)(p + 64 + 12 * n)};
+}
+
+// TSFX_FLAG_DEFER_CHECK (tsfx.h "Deferred input check"): the validation pass, the groups on the private views (CSR) or
+// on the input as it is (dense), then the NaN rows and the report.  Only enqueues: a prepared shape needs no allocation.
+static int extract_deferred(tsfx_ctx* ctx, const tsfx_plan* plan, SeriesRef R, int64_t n_values, int max_len, double* out,
+                            uint32_t flags, int ld) {
+    if (flags & (TSFX_FLAG_CHECK_DEVICE_INPUT | TSFX_FLAG_IMPUTE))
+        return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_DEFER_CHECK excludes TSFX_FLAG_CHECK_DEVICE_INPUT and TSFX_FLAG_IMPUTE");
+    if (!ctx->status) return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_DEFER_CHECK needs a status buffer (tsfx_set_status)");
+    if (max_len < 1) return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_DEFER_CHECK needs the longest series (tsfx_set_max_len_hint)");
+    if (R.n_series > ctx->prep_series || max_len > ctx->prep_len)
+        return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_DEFER_CHECK: " + std::to_string(R.n_series) + " series of up to " +
+                                             std::to_string(max_len) + " samples, more than tsfx_prepare made ready");
+    if (n_values < 1) return fail(ctx, TSFX_E_INVALID, "TSFX_FLAG_DEFER_CHECK: no values");
+    const DeferBufs B = defer_bufs(ctx);
+    const bool csr = R.begin != nullptr;
+    CK(cudaMemsetAsync(B.first, 0, 3 * sizeof(unsigned long long), ctx->stream));
+    CK(defer_check(R.values, n_values, R.begin, R.len, R.n_series, max_len, csr ? B.vbegin : nullptr, B.vlen, B.reject,
+                   B.first, ctx->stream));
+    if (csr) { R.begin = B.vbegin; R.len = B.vlen; }
+    if (int rc = run_groups(ctx, plan, R, max_len, out, flags, ld)) return rc;
+    CK(defer_finish(out, R.n_series, plan->ncols, ld, B.reject, B.first, ctx->status, ctx->stream));
+    ctx->launches += 2;
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_prepare(tsfx_ctx* ctx, const tsfx_plan* plan, int64_t n_series, int32_t max_len) {
+    int rc = check_args(ctx, plan, nullptr, nullptr, 0);
+    if (rc) return rc;
+    if (n_series < 1 || max_len < 1) return fail(ctx, TSFX_E_INVALID, "tsfx_prepare: n_series and max_len must be >= 1");
+    CK(cudaSetDevice(ctx->device));
+    if ((rc = check_lengths(ctx, plan, max_len))) return rc;
+    if ((rc = reserve_groups(ctx, plan, n_series, max_len))) return rc;
+    const int64_t n = std::max(n_series, ctx->prep_series);
+    CK(ctx->defer.reserve(defer_bytes(n)));
+    ctx->prep_series = n;
+    ctx->prep_len = std::max(ctx->prep_len, (int)max_len);
+    CK(cudaStreamSynchronize(ctx->stream));     // the tables are filled before a captured call, which cannot wait for them
+    return TSFX_OK;
+}
+
+extern "C" int tsfx_set_status(tsfx_ctx* ctx, int64_t* status) {
+    if (!ctx) return TSFX_E_INVALID;
+    ctx->status = status;
+    return TSFX_OK;
+}
+
+extern "C" int32_t tsfx_plan_max_len(const tsfx_feature_desc* descs, int32_t n_descs) {
+    if (n_descs < 0 || (n_descs > 0 && !descs)) return TSFX_E_INVALID;
+    int32_t m = 0x7fffffff;
+    for (int i = 0; i < n_descs; ++i) {
+        if (descs[i].calc < 0 || descs[i].calc >= TSFX_N_CALCS) return TSFX_E_INVALID;
+        m = std::min(m, (int32_t)group_max_len(group_of(descs[i].calc)));
+    }
+    return m;
+}
+
 // row stride of a device-pointer call's `out` (tsfx_set_out_ld)
 static int device_out_ld(tsfx_ctx* ctx, const tsfx_plan* plan, uint32_t flags, int* ld) {
     *ld = ctx->out_ld > 0 ? ctx->out_ld : plan->ncols;
@@ -963,6 +1056,7 @@ extern "C" int tsfx_extract_csr(tsfx_ctx* ctx, const tsfx_plan* plan, const floa
         int ld = 0;
         rc = device_out_ld(ctx, plan, flags, &ld);
         if (rc) return rc;
+        if (flags & TSFX_FLAG_DEFER_CHECK) return extract_deferred(ctx, plan, R, n_values, ctx->max_len_hint, out, flags, ld);
         if (flags & TSFX_FLAG_CHECK_DEVICE_INPUT) {
             rc = check_device_input(ctx, values, n_values, begin, len, n_series, &max_len);
             if (rc) return rc;
@@ -1023,6 +1117,7 @@ extern "C" int tsfx_extract_dense(tsfx_ctx* ctx, const tsfx_plan* plan, const fl
         int ld = 0;
         rc = device_out_ld(ctx, plan, flags, &ld);
         if (rc) return rc;
+        if (flags & TSFX_FLAG_DEFER_CHECK) return extract_deferred(ctx, plan, R, n_series * (int64_t)len, len, out, flags, ld);
         if (flags & TSFX_FLAG_CHECK_DEVICE_INPUT) {
             int max_len = len;
             rc = check_device_input(ctx, values, n_series * (int64_t)len, nullptr, nullptr, n_series, &max_len);

@@ -939,6 +939,68 @@ cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, c
     return cudaGetLastError();
 }
 
+// One warp per series, as k_check_views, but every series gets its own verdict instead of the call getting one
+__global__ void k_defer_check(const float* __restrict__ values, int64_t n_values, const int64_t* __restrict__ begin,
+                              const int32_t* __restrict__ len, int64_t n_series, int32_t max_len, int64_t* __restrict__ vbegin,
+                              int32_t* __restrict__ vlen, uint8_t* __restrict__ reject, unsigned long long* first) {
+    const int lane = threadIdx.x & 31;
+    int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (; w < n_series; w += n_warps) {                  // warp-uniform
+        int64_t b = w * (int64_t)max_len;
+        int32_t l = max_len;
+        int why = 0;
+        if (begin) {
+            b = begin[w];
+            l = len[w];
+            if (l < 1 || b < 0 || b > n_values - l) why = DEFER_VIEW;
+            else if (l > max_len) why = DEFER_LONG;
+        }
+        if (!why) {
+            int nan = 0;
+            for (int32_t i = lane; i < l; i += 32) { const float v = values[b + i]; nan |= v != v; }
+            if (__any_sync(0xffffffffu, nan)) why = DEFER_NAN;
+        }
+        if (lane == 0) {
+            reject[w] = (uint8_t)why;
+            if (why) atomicMax(first + (why - 1), (unsigned long long)(n_series - w));
+            if (vbegin) { vbegin[w] = why ? 0 : b; vlen[w] = why ? 1 : l; }
+        }
+    }
+}
+
+cudaError_t defer_check(const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
+                        int64_t n_series, int32_t max_len, int64_t* vbegin, int32_t* vlen, uint8_t* reject,
+                        unsigned long long* first, cudaStream_t st) {
+    if (n_series <= 0) return cudaSuccess;
+    k_defer_check<<<grid_for(n_series * 32, 256), 256, 0, st>>>(d_values, n_values, d_begin, d_len, n_series, max_len,
+                                                                vbegin, vlen, reject, first);
+    return cudaGetLastError();
+}
+
+__global__ void k_defer_finish(double* __restrict__ out, int64_t n_series, int n_cols, int ld, const uint8_t* __restrict__ reject,
+                               const unsigned long long* __restrict__ first, int64_t* status) {
+    if (blockIdx.x == 0 && threadIdx.x == 0) {           // one thread: the calls on a status buffer are stream-ordered
+        const int64_t call = status[TSFX_STATUS_CALLS] + 1;
+        status[TSFX_STATUS_CALLS] = call;
+        if (status[TSFX_STATUS_BAD] == 0 && (first[0] | first[1] | first[2])) {
+            status[TSFX_STATUS_BAD] = call;
+            for (int r = 0; r < 3; ++r) status[TSFX_STATUS_VIEW + r] = first[r] ? n_series - (int64_t)first[r] : -1;
+        }
+    }
+    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; s < n_series; s += stride)
+        if (reject[s])
+            for (int c = 0; c < n_cols; ++c) out[s * ld + c] = __longlong_as_double(0x7ff8000000000000LL);
+}
+
+cudaError_t defer_finish(double* out, int64_t n_series, int n_cols, int ld, const uint8_t* reject,
+                         const unsigned long long* first, int64_t* status, cudaStream_t st) {
+    k_defer_finish<<<grid_for(n_series, 256), 256, 0, st>>>(out, n_series, n_cols, ld, reject, first, status);
+    return cudaGetLastError();
+}
+
 int csr_max_len(CsrWorkspace& W, const int32_t* d_len, int64_t n, cudaStream_t st, int* out) {
     std::string* msg = nullptr;
     CKE(W.reserve(S_FLAG, 64), "alloc");

@@ -177,4 +177,18 @@ cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, c
 void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
                      int64_t n_series, cudaStream_t st);
 
+// Deferred input check (TSFX_FLAG_DEFER_CHECK), one launch: per series (dense: row s of max_len samples at
+// values + s * max_len, begin == nullptr; CSR: the caller's view) its reject reason into reject[s] (DEFER_VIEW, DEFER_LONG
+// or DEFER_NAN, 0: none) and, per reason r, n_series - s of the first rejected series into first[r - 1] (atomicMax,
+// zeroed by the caller).  CSR: the private view of every series into vbegin / vlen, (0, 1) for a rejected one.
+enum { DEFER_VIEW = 1, DEFER_LONG, DEFER_NAN };
+cudaError_t defer_check(const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
+                        int64_t n_series, int32_t max_len, int64_t* vbegin, int32_t* vlen, uint8_t* reject,
+                        unsigned long long* first, cudaStream_t st);
+
+// After the groups of a deferred-check call: NaN in every column of every rejected series (out[s * ld + c], c < n_cols),
+// then the call's report into the caller's status words (tsfx.h TSFX_STATUS_*).
+cudaError_t defer_finish(double* out, int64_t n_series, int n_cols, int ld, const uint8_t* reject,
+                         const unsigned long long* first, int64_t* status, cudaStream_t st);
+
 }  // namespace tsfx

@@ -34,6 +34,14 @@ cuts the staged series into consecutive packages of sub_length rows (views again
 is make_forecasting_frame(x, ...) extracted, with its target vector aligned to the rows of X: the rolled call on one
 series whose windows tsfx_roll_staged (TSFX_FLAG_FORECAST) shortens by their last row, and whose targets it reports as
 input row numbers that torch gathers from x.
+
+    ex = DeviceExtractor(4096, length=256)                              # or max_length=... for CSR views
+    X = ex(values, out=X)                                               # enqueues only: no host synchronisation
+    ex.check()                                                          # raises what extract_features_device would have
+
+is extract_features_device prepared once for a batch shape: each call only enqueues work on torch's current stream, so
+it overlaps other work and can be captured in a CUDA graph.  Its input is checked on the device (TSFX_FLAG_DEFER_CHECK):
+rejected series come out as NaN rows and check() raises the error at a sync point the caller chooses.
 """
 import numbers
 
@@ -183,6 +191,145 @@ def extract_features_device(values, begin=None, length=None, *, default_fc_param
         impute_function(df)
         X.copy_(torch.from_numpy(df.to_numpy(dtype=np.float64)))
     return X, columns
+
+
+class DeviceExtractor:
+    """extract_features_device prepared for one batch shape, for calls that only enqueue work.
+
+        ex = DeviceExtractor(batch_size, length=L)            # dense [n, L] or channels-last [n, L, K], n <= batch_size
+        ex = DeviceExtractor(batch_size, max_length=M)        # CSR views (values, begin, length), each <= M samples
+        X = ex(values, out=None)  /  X = ex(values, begin, length, out=None)
+        ex.check()
+
+    kinds, default_fc_parameters and kind_to_fc_parameters are as for extract_features_device (kinds default: one kind,
+    named 0); `columns` are the names it gives.  device: the CUDA device of the inputs (default: the current one).
+
+    The plans are compiled, their length limits checked against length / max_length (ValueError), and every working
+    buffer sized once, here.  The extractor owns a private library context, so calls never share scratch with the eager
+    API or another extractor (and may be replayed from a CUDA graph on any stream): 256 MB of working memory (1 GB when
+    length / max_length exceeds 1 024) plus the per-kind staging matrices (batch_size x staged columns x 8 bytes) and 13
+    bytes per series of check buffers.  Calls on one extractor are stream-ordered: use one extractor per concurrent
+    stream.
+
+    A call checks the tensors' shapes, dtypes and devices, and `out`, at once (TypeError / ValueError, nothing enqueued).
+    It then enqueues on torch's current stream, with no host synchronisation, no allocation in the library and no read
+    of device memory on the host; float64, float16 and bfloat16 are rounded to float32 on the device.  The data are
+    checked on the device: a series with a NaN value, an invalid view (len < 1, begin < 0, begin + len > R) or a view
+    longer than max_length is rejected.  Every other row is what extract_features_device gives (bit for bit for dense
+    input and for views whose longest equals max_length; a shorter longest view may select other kernel variants, which
+    agree within the oracle parity); a rejected row is NaN in every column of its kind.  check() synchronises the device
+    and raises the ValueError extract_features_device would have raised for the first call since the last check() that
+    rejected a series, then clears that state.  impute_function is not offered (imputation synchronises): impute X
+    afterwards."""
+
+    def __init__(self, batch_size, length=None, max_length=None, *, kinds=None, default_fc_parameters=None,
+                 kind_to_fc_parameters=None, device=None):
+        import torch
+        if (length is None) == (max_length is None):
+            raise ValueError("give exactly one of length (dense input) or max_length (CSR views)")
+        for name, v in (("batch_size", batch_size), ("length", length), ("max_length", max_length)):
+            if v is not None and (not isinstance(v, numbers.Integral) or not 1 <= v <= 0x7fffffff):
+                raise ValueError("%s must be an integer in 1 .. 2^31 - 1, got %r" % (name, v))
+        self.batch_size, self.length, self.max_length = int(batch_size), length, max_length
+        kinds = [0] if kinds is None else list(kinds)
+        _layout(torch.empty((0, 1, len(kinds)), device="meta"), None, None, kinds)      # the kinds' names, as a call checks them
+        self.kinds = kinds
+        self._plans, self.columns = _plans(kinds, default_fc_parameters, kind_to_fc_parameters)
+        longest = length if length is not None else max_length
+        for kind, plan in zip(kinds, self._plans):
+            limit = _lib.plan_max_len(plan)
+            if longest > limit:
+                raise ValueError("series of %d samples exceed the limit of kind %r's settings (%d samples)" % (longest, kind, limit))
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != "cuda":
+            raise ValueError("device must be a CUDA device, got %s" % self.device)
+        self._open()
+
+    def _open(self):
+        """The private context, its prepared plans and the status words (tsfx.h "Deferred input check")."""
+        import torch
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self._ctx = _lib.Context(self.device.index)
+        self._dps = [None if p.n_cols == 0 else _device_plan(self._ctx, p) for p in self._plans]
+        for dp in self._dps:
+            if dp is not None:
+                dp.prepare(self.batch_size, self.length or self.max_length)
+        self._status = torch.zeros(_lib.STATUS_WORDS, dtype=torch.int64, device=self.device)
+        self._ctx.set_status(self._status.data_ptr())
+
+    def __call__(self, values, begin=None, length=None, out=None):
+        import torch
+        n, _, csr = _layout(values, begin, length, self.kinds)
+        if csr != (self.max_length is not None):
+            raise ValueError("this extractor takes %s" % ("CSR views (values, begin, length)" if self.max_length is not None
+                                                           else "dense [n, length] or [n, length, K] values"))
+        if n > self.batch_size:
+            raise ValueError("%d series, the extractor was built for at most %d" % (n, self.batch_size))
+        if not csr and values.shape[1] != self.length:
+            raise ValueError("series of %d samples, the extractor was built for length=%d" % (values.shape[1], self.length))
+        if csr and n > 0 and values.shape[0] == 0:
+            raise ValueError("values is empty")
+        width = len(self.columns)
+        if out is not None:
+            _check_out(out, n, width)
+        dev = self.device
+        for name, t in (("values", values), ("begin", begin), ("length", length), ("out", out)):
+            if t is not None and t.device != dev:
+                raise ValueError("%s is on %s, the extractor on %s" % (name, t.device, dev))
+        with torch.cuda.device(dev):
+            X = out if out is not None else torch.empty((n, width), dtype=torch.float64, device=dev)
+            if n == 0 or width == 0:
+                return X
+            v = values if values.dtype == torch.float32 else values.to(torch.float32)
+            if csr:
+                b = begin.contiguous()
+                # int64 lengths beyond int32 become lengths the check rejects, never wrapped-around valid ones
+                ln = length.contiguous() if length.dtype == torch.int32 else length.clamp(0, 0x7fffffff).to(torch.int32)
+            ctx = self._ctx
+            scratch = None
+            with ctx.lock:
+                # the context stays bound to the stream it last ran on: rebinding it after a capture would order a
+                # stream outside the graph after work inside it
+                ctx.set_stream(torch.cuda.current_stream(dev).cuda_stream or _lib.STREAM_LEGACY)
+                ctx.set_out_ld(X.stride(0))
+                c0 = 0
+                for k, dp in enumerate(self._dps):
+                    if dp is None:
+                        continue
+                    if v.ndim == (2 if csr else 3):             # channels-last: this kind's values, contiguous
+                        scratch = torch.empty(v.shape[:-1], dtype=torch.float32, device=dev) if scratch is None else scratch
+                        col = scratch.copy_(v[..., k])
+                    else:
+                        col = v.contiguous()
+                    o = X.data_ptr() + c0 * 8
+                    if csr:
+                        dp.extract_csr_device(col.data_ptr(), col.shape[0], b.data_ptr(), ln.data_ptr(), n, o,
+                                              max_len=self.max_length, deferred=True)
+                    else:
+                        dp.extract_dense_device(col.data_ptr(), n, col.shape[1], o, deferred=True)
+                    c0 += dp.n_cols
+        return X
+
+    def check(self):
+        """Synchronises the device; raises the ValueError of the first call since the last check() that rejected a
+        series (then forgets it)."""
+        import torch
+        torch.cuda.synchronize(self.device)
+        st = self._status.cpu().tolist()
+        bad = st[_lib.STATUS_BAD]
+        if bad == 0:
+            return
+        self._status[_lib.STATUS_BAD] = 0
+        torch.cuda.synchronize(self.device)
+        active = [k for k, dp in zip(self.kinds, self._dps) if dp is not None]
+        kind = active[(bad - 1) % len(active)]                # every call makes one library call per kind with columns
+        if st[_lib.STATUS_VIEW] >= 0:
+            raise ValueError("series %d has an invalid (begin, len): len < 1, begin < 0 or begin + len > n_values"
+                             % st[_lib.STATUS_VIEW])
+        if st[_lib.STATUS_LONG] >= 0:
+            raise ValueError("series %d is longer than max_length=%d" % (st[_lib.STATUS_LONG], self.max_length))
+        raise ValueError("Column must not contain NaN values: {} (first in series {})".format(kind, st[_lib.STATUS_NAN]))
 
 
 def _long_layout(ids, values, sort, kind, kinds, times, need_ids=True):
