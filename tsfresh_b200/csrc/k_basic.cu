@@ -6,7 +6,8 @@
 // ST[32] (shared statistics read by the lane-parallel finishers), altS[6 nalt] (regression sums per
 // agg_linear_trend key); in front of the per-warp regions one CTA-wide copy of the descriptor table.  Two CTAs of 12
 // warps per SM walk the descriptor list in lock step (instruction-cache sharing); the 41 lag products run on the FP64
-// tensor cores (lag_products_dmma).  Calculators restated (feature_calculators.py line numbers in
+// tensor cores (lag_products_dmma); linear_trend's p-value is finished by k_basic_pvalue, one thread per series, after
+// the kernel.  Calculators restated (feature_calculators.py line numbers in
 // include/tsfx.h): every "class M" and "class O" row of SURVEY.md section 8a, plus linear_trend_timewise.
 #include "tsfx_common.cuh"
 #include "tsfx_math.cuh"
@@ -841,8 +842,12 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
                     sxx = wsum(sxx) / dn;
                     sxy = wsum(sxy) / dn;
                     const LinReg fit = m_linregress(dn, tm, M.mean, sxx, M.var, sxy);
+                    // the p-value column gets the t statistic: k_basic_pvalue turns it into the p-value
                     if (live)
-                        for (int t = lane; t < run; t += 32) orow[j + t] = m_linreg_pick(fit, sdesc[j + t].attr);
+                        for (int t = lane; t < run; t += 32) {
+                            const int attr = sdesc[j + t].attr;
+                            orow[j + t] = attr == TSFX_LR_PVALUE ? fit.tstat : m_linreg_pick(fit, attr);
+                        }
                     break;
                 }
                 case TSFX_LINEAR_TREND_TIMEWISE: {
@@ -968,6 +973,18 @@ __global__ void __launch_bounds__(WPC * 32, (WPC == 8 ? 3 : (WPC == 12 ? 2 : 1))
     }
 }
 
+// linear_trend's p-value, one thread per series: 2 stdtr(n - 2, -|t|) of the t statistic k_basic left in the column.
+// The incomplete-beta continued fraction is a serial chain of up to 400 steps with four divisions each; inside k_basic
+// it ran on one lane while the other 31 lanes and the CTA's other warps (held by the per-trip barrier) waited.  Same
+// function and same operands (t from the column, df = n - 2.0 as m_linregress forms it), so the same bits.
+__global__ void __launch_bounds__(256) k_basic_pvalue(SeriesRef R, double* out, int ncols, int col) {
+    for (int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; s < R.n_series; s += (int64_t)gridDim.x * blockDim.x) {
+        const int n = R.begin ? R.len[s] : R.dense_len;
+        double* o = out + (size_t)s * ncols + col;
+        *o = m_student_two_sided(*o, (double)n - 2.0);
+    }
+}
+
 bool basic_finisher_calc(int calc) { return basic_is_finisher(calc); }
 
 // ------------------------------------------------------------------------------------------ launcher
@@ -1009,7 +1026,10 @@ cudaError_t launch_basic(const BasicArgs& A0, bool vocab, int max_len, cudaStrea
         constexpr bool GL = decltype(g)::global;
         return vocab ? launch_kernel(k_basic<W, GL, true>, G, st, A) : launch_kernel(k_basic<W, GL, false>, G, st, A);
     };
-    TSFX_LAUNCH_DECLARED(TSFX_GEOMS_BASIC, "basic", G, variant, launch);
+    const cudaError_t e = [&]() -> cudaError_t { TSFX_LAUNCH_DECLARED(TSFX_GEOMS_BASIC, "basic", G, variant, launch); }();
+    if (e != cudaSuccess || A.lt_pcol < 0) return e;
+    return launch_fixed(k_basic_pvalue, 256, 256, 0, (int64_t)sm_count * 16, A.R.n_series, st, A.R, A.out, A.ncols,
+                        A.lt_pcol);
 }
 
 }  // namespace tsfx

@@ -661,6 +661,9 @@ extern "C" int tsfx_plan_create(tsfx_ctx* ctx, const tsfx_feature_desc* descs, i
             P->basic_vocab = true;
     }
     B.dec = ctx->d_dec;
+    B.lt_pcol = -1;
+    for (int q = 0; q < (int)P->host[G_BASIC].size(); ++q)
+        if (P->host[G_BASIC][q].calc == TSFX_LINEAR_TREND && P->host[G_BASIC][q].attr == TSFX_LR_PVALUE) B.lt_pcol = q;
     SortedArgs& S = P->sorted;
     group(S, G_SORTED);
     S.nscr = even(4 * (friedrich_r + 2) + 16);

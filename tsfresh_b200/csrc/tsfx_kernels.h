@@ -182,6 +182,8 @@ struct BasicArgs : GroupArgs {
     int lag_needed;      // largest lag product any descriptor reads (0 = none)
     int pacf_off;        // offset (doubles) of the pacf staging area inside lagS
     const double* dec;   // device table d*10^k, k = TSFX_DEC_MIN..TSFX_DEC_MAX, 9 per decade
+    int lt_pcol;         // staging column of linear_trend's p-value (k_basic leaves the t statistic there and
+                         // k_basic_pvalue finishes it, see k_basic.cu); -1: the plan has no such column
 };
 // vocab: the plan has a column basic_vocabulary (k_basic.cu) finishes: agg_autocorrelation with a reducer other than
 // mean / median / var / std, or linregress attr intercept_stderr
