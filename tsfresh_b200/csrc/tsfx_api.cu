@@ -1538,7 +1538,7 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
                                        int32_t* max_len_per_kind, uint32_t flags) {
     if (!ctx) return TSFX_E_INVALID;
     StackedWorkspace& S = ctx->stacked;
-    S.valid = false;
+    S.pending = false;
     ctx->launches = 0;
     ctx->n_kernels = 0;
     if (!(flags & TSFX_FLAG_DEVICE_PTRS)) return fail(ctx, TSFX_E_INVALID, "tsfx_stage_long_stacked takes device pointers");
@@ -1555,9 +1555,7 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
     S.d_keys = nullptr;
     S.d_src = nullptr;
     S.has_keys = false;
-    S.rolled = false;
-    S.packaged = false;
-    S.forecast = false;
+    S.staged = Staged::Rows;
     if (n_rows > 0) {
         std::string msg;
         int rc = stacked_stage(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values, kind_codes,
@@ -1577,7 +1575,7 @@ extern "C" int tsfx_stage_long_stacked(tsfx_ctx* ctx, const int64_t* ids, const 
         }
     }
     *n_ids_out = S.n_union;
-    S.valid = true;
+    S.pending = true;
     return TSFX_OK;
 }
 
@@ -1587,8 +1585,8 @@ extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans,
     StackedWorkspace& S = ctx->stacked;
     ctx->launches = 0;
     ctx->n_kernels = 0;
-    if (!S.valid) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: no rows staged (tsfx_stage_long_stacked)");
-    S.valid = false;
+    if (!S.pending) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: no rows staged (tsfx_stage_long_stacked)");
+    S.pending = false;
     const int64_t U = S.n_union;
     if (U == 0) return TSFX_OK;
     if (!plans || !out_ids) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_staged: bad arguments");
@@ -1642,26 +1640,59 @@ extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans,
     return TSFX_OK;
 }
 
+// The steps tsfx_roll_staged and tsfx_sub_staged share before they replace the staged series by pieces of them (`to`):
+// the state check, then the caller's argument error `bad` (nullptr: none), the outputs zeroed and the stage consumed
+// until the call succeeds.  *empty: no rows are staged, so the call is complete.
+static int regroup_begin(tsfx_ctx* ctx, const char* call, Staged to, const char* bad, int64_t* n_rows_out,
+                         int32_t* max_len_per_kind, bool* empty) {
+    StackedWorkspace& S = ctx->stacked;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (!S.pending || S.staged != Staged::Rows)
+        return fail(ctx, TSFX_E_INVALID, std::string(call) + ": no unrolled, unpackaged rows staged (tsfx_stage_long_stacked)");
+    if (bad) return fail(ctx, TSFX_E_INVALID, bad);
+    S.pending = false;
+    *n_rows_out = 0;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
+    *empty = S.n_union == 0;
+    if (*empty) { S.staged = to; S.pending = true; return TSFX_OK; }
+    CK(cudaSetDevice(ctx->device));
+    return TSFX_OK;
+}
+
+// The steps they share once the regrouping is enqueued: the new stage state, one synchronisation, then the pieces'
+// sizes published and the stage ready for tsfx_extract_staged.
+static int regroup_end(tsfx_ctx* ctx, Staged to, int64_t* n_rows_out, int32_t* max_len_per_kind) {
+    StackedWorkspace& S = ctx->stacked;
+    S.staged = to;
+    CK(cudaStreamSynchronize(ctx->stream));
+    const StackedInfo& I = *S.h_info;
+    if (I.dup_names)
+        return fail(ctx, TSFX_E_INVALID, "two windows of one kind have the same name (id, sort key): the sort keys tie at "
+                                         "the rows that name them");
+    S.n_union = I.n_union;
+    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = I.kind_max_len[k];
+    *n_rows_out = S.n_union;
+    S.pending = true;
+    return TSFX_OK;
+}
+
 extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                                 int64_t* n_rows_out, int32_t* max_len_per_kind, uint32_t flags) {
     if (!ctx) return TSFX_E_INVALID;
     const bool forecast = (flags & TSFX_FLAG_FORECAST) != 0;
+    const Staged to = forecast ? Staged::ForecastWindows : Staged::Windows;
     StackedWorkspace& S = ctx->stacked;
-    ctx->launches = 0;
-    ctx->n_kernels = 0;
-    if (!S.valid || S.rolled || S.packaged)
-        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: no unrolled, unpackaged rows staged (tsfx_stage_long_stacked)");
+    const char* bad = nullptr;
     if (!n_rows_out || !max_len_per_kind || rolling_direction == 0 || max_timeshift < 0 || min_timeshift < 0)
-        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: bad arguments");
-    if (S.has_keys && !S.d_keys)
-        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: the rows were staged without TSFX_FLAG_KEEP_SORT_KEYS");
-    if (forecast && S.n_union > 0 && !S.d_src)
-        return fail(ctx, TSFX_E_INVALID, "tsfx_roll_staged: TSFX_FLAG_FORECAST needs rows staged with TSFX_FLAG_KEEP_ROW_NUMBERS");
-    S.valid = false;
-    *n_rows_out = 0;
-    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
-    if (S.n_union == 0) { S.rolled = true; S.forecast = forecast; S.valid = true; return TSFX_OK; }
-    CK(cudaSetDevice(ctx->device));
+        bad = "tsfx_roll_staged: bad arguments";
+    else if (S.has_keys && !S.d_keys)
+        bad = "tsfx_roll_staged: the rows were staged without TSFX_FLAG_KEEP_SORT_KEYS";
+    else if (forecast && S.n_union > 0 && !S.d_src)
+        bad = "tsfx_roll_staged: TSFX_FLAG_FORECAST needs rows staged with TSFX_FLAG_KEEP_ROW_NUMBERS";
+    bool empty = false;
+    if (int rc = regroup_begin(ctx, "tsfx_roll_staged", to, bad, n_rows_out, max_len_per_kind, &empty)) return rc;
+    if (empty) return TSFX_OK;
     const StackedInfo& I = *S.h_info;
     // the shifts are anchored to the longest (kind, id) series; a window never has more rows than its series, and a
     // series of L rows has at most one window per shift <= L
@@ -1677,15 +1708,7 @@ extern "C" int tsfx_roll_staged(tsfx_ctx* ctx, int32_t rolling_direction, int32_
     int rc = stacked_roll(S, ctx->csr, rolling_direction, max_timeshift, min_timeshift, Lmax, bound, forecast, ctx->stream,
                           &msg);
     if (rc) return fail(ctx, rc, msg);
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (I.dup_names)
-        return fail(ctx, TSFX_E_INVALID, "two windows of one kind have the same name (id, sort key): the sort keys tie at "
-                                         "the rows that name them");
-    S.n_union = I.n_union;
-    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = I.kind_max_len[k];
-    *n_rows_out = S.n_union;
-    S.valid = true;
-    return TSFX_OK;
+    return regroup_end(ctx, to, n_rows_out, max_len_per_kind);
 }
 
 extern "C" int tsfx_sub_staged(tsfx_ctx* ctx, int64_t sub_length, int64_t* n_rows_out, int32_t* max_len_per_kind,
@@ -1693,16 +1716,11 @@ extern "C" int tsfx_sub_staged(tsfx_ctx* ctx, int64_t sub_length, int64_t* n_row
     (void)flags;
     if (!ctx) return TSFX_E_INVALID;
     StackedWorkspace& S = ctx->stacked;
-    ctx->launches = 0;
-    ctx->n_kernels = 0;
-    if (!S.valid || S.rolled || S.packaged)
-        return fail(ctx, TSFX_E_INVALID, "tsfx_sub_staged: no unrolled, unpackaged rows staged (tsfx_stage_long_stacked)");
-    if (!n_rows_out || !max_len_per_kind || sub_length < 1) return fail(ctx, TSFX_E_INVALID, "tsfx_sub_staged: bad arguments");
-    S.valid = false;
-    *n_rows_out = 0;
-    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = 0;
-    if (S.n_union == 0) { S.packaged = true; S.valid = true; return TSFX_OK; }
-    CK(cudaSetDevice(ctx->device));
+    const char* bad = !n_rows_out || !max_len_per_kind || sub_length < 1 ? "tsfx_sub_staged: bad arguments" : nullptr;
+    bool empty = false;
+    if (int rc = regroup_begin(ctx, "tsfx_sub_staged", Staged::Packages, bad, n_rows_out, max_len_per_kind, &empty))
+        return rc;
+    if (empty) return TSFX_OK;
     const StackedInfo& I = *S.h_info;
     // every series has fewer than 2^31 rows, so a longer sub_length gives the same packages: whole series
     const int32_t L = (int32_t)std::min<int64_t>(sub_length, 0x7fffffff);
@@ -1717,18 +1735,13 @@ extern "C" int tsfx_sub_staged(tsfx_ctx* ctx, int64_t sub_length, int64_t* n_row
     std::string msg;
     int rc = stacked_sub(S, ctx->csr, L, bound, ctx->stream, &msg);
     if (rc) return fail(ctx, rc, msg);
-    CK(cudaStreamSynchronize(ctx->stream));
-    S.n_union = I.n_union;
-    for (int k = 0; k < S.n_kinds; ++k) max_len_per_kind[k] = I.kind_max_len[k];
-    *n_rows_out = S.n_union;
-    S.valid = true;
-    return TSFX_OK;
+    return regroup_end(ctx, Staged::Packages, n_rows_out, max_len_per_kind);
 }
 
 extern "C" int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys) {
     if (!ctx) return TSFX_E_INVALID;
     StackedWorkspace& S = ctx->stacked;
-    if (!S.rolled && !S.packaged)
+    if (S.staged == Staged::Rows)
         return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: no windows or packages staged (tsfx_roll_staged, tsfx_sub_staged)");
     if (S.n_union == 0) return TSFX_OK;
     if (!out_keys) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_row_keys: NULL out_keys");
@@ -1740,7 +1753,7 @@ extern "C" int tsfx_staged_row_keys(tsfx_ctx* ctx, void* out_keys) {
 extern "C" int tsfx_staged_targets(tsfx_ctx* ctx, int64_t* out_rows) {
     if (!ctx) return TSFX_E_INVALID;
     StackedWorkspace& S = ctx->stacked;
-    if (!S.rolled || !S.forecast)
+    if (S.staged != Staged::ForecastWindows)
         return fail(ctx, TSFX_E_INVALID, "tsfx_staged_targets: no forecasting windows staged (tsfx_roll_staged, TSFX_FLAG_FORECAST)");
     if (S.n_union == 0) return TSFX_OK;
     if (!out_rows) return fail(ctx, TSFX_E_INVALID, "tsfx_staged_targets: NULL out_rows");

@@ -283,9 +283,9 @@ int csr_sort_pass(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys,
 // ---------------------------------------------------------------------------------------------------------------------
 // stacked long format (tsfx_csr.h)
 enum { T_CODE = 0, T_UROW, T_COUNTS, T_TEMP, T_VALS, T_SROW, T_TIMES, T_BEGIN, T_LEN, T_ROW, T_UID, T_INFO, T_KEYS,
-       // stacked_roll: per-series window offsets, per-window begin / len / union row / parent id / name, scanned name
-       // flags, union windows' names
-       R_OFF, R_BEGIN, R_LEN, R_ROW, R_ID, R_KEY, R_SCAN, R_UID, R_UKEY,
+       // stacked_roll / stacked_sub: per-series piece offsets, per-piece (window or package) begin / len / union row /
+       // parent id / name key, scanned name flags, union pieces' names
+       G_OFF, G_BEGIN, G_LEN, G_ROW, G_ID, G_KEY, G_SCAN, G_UID, G_UKEY,
        // stacked_sub: begin / len / union row of every package in union order inside its kind
        P_BEGIN, P_LEN, P_ROW,
        // input row number of every staged row; stacked_roll with forecast: target row of every window and union window
@@ -313,7 +313,13 @@ void StackedWorkspace::release() {
     h_info = nullptr; d_info = nullptr;
     d_values = nullptr; d_times = nullptr; d_begin = nullptr; d_len = nullptr; d_row = nullptr; d_uid = nullptr;
     d_keys = nullptr; d_ukey = nullptr; d_src = nullptr; d_utarget = nullptr;
-    valid = false; rolled = false; packaged = false; forecast = false;
+    staged = Staged::Rows; pending = false;
+}
+
+// the device's sizes and flags (d_info) to the host's copy (h_info), asynchronously: the caller synchronises
+static int stacked_publish(StackedWorkspace& S, cudaStream_t st, std::string* msg) {
+    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
+    return TSFX_OK;
 }
 
 #define STACK_TILE 4096          // rows per CTA of the counting sort
@@ -472,10 +478,6 @@ __global__ void k_stack_finish(const CsrInfo* csr, StackedInfo* info) {
 int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
                   const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
                   int64_t n, bool keep_keys, bool keep_rows, cudaStream_t st, std::string* msg) {
-    S.valid = false;
-    S.rolled = false;
-    S.packaged = false;
-    S.forecast = false;
     S.n_kinds = n_kinds;
     S.has_keys = d_keys != nullptr;
     S.keys_f64 = d_keys && keys_f64;
@@ -539,12 +541,12 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     k_stack_lengths<<<grid_for(n / 4 + 1, 256), 256, 0, st>>>(urow, n_pad, n_kinds, S.d_begin, S.d_len, S.d_info);
     k_stack_finish<<<1, 1, 0, st>>>(W.d_info, S.d_info);
     CKE(cudaGetLastError(), "series kernels");
-    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
-    return TSFX_OK;
+    return stacked_publish(S, st, msg);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// rolled windows of the staged series (stacked_roll)
+// rolled windows of the staged series (stacked_roll), and the regrouping that fixed-length packages (stacked_sub)
+// share with them: pieces of the staged series replace them, named, with a union of the names
 
 // kind whose series range holds series s (the last of kinds that start at the same series is the only one with series)
 __device__ __forceinline__ int kind_of_series(const StackedInfo* info, int n_kinds, int64_t s) {
@@ -561,27 +563,47 @@ __device__ __forceinline__ uint64_t window_name(const uint64_t* __restrict__ key
     return keys_f64 && k == 0x8000000000000000ull ? 0ull : k;
 }
 
-// windows of every series into cnt[s]; each kind's longest window into info->kind_max_len (zeroed by the caller).  The
-// window lengths are monotone in the shift, so a series' longest window is its first or its last.  Forecast: every window
-// loses its last row.
+// A cut gives the number of pieces of a series of L rows and, in *longest, its longest piece.  Windows: the window
+// lengths are monotone in the shift, so a series' longest window is its first or its last; Forecast: every window loses
+// its last row.
 template <bool Forecast>
-__global__ void k_roll_count(const int32_t* __restrict__ len, int64_t n_series, RollSpec R, int n_kinds,
-                             int32_t* __restrict__ cnt, StackedInfo* info) {
+struct RollCut {
+    RollSpec R;
+    __device__ int32_t operator()(int32_t L, int32_t* longest) const {
+        int32_t t0, lo;
+        const int64_t n = roll_kept(R, L, &t0);
+        *longest = 0;
+        if (n > 0) {
+            const int32_t first = roll_window(R, L, t0, &lo);
+            const int32_t last = roll_window(R, L, (int32_t)(t0 + (n - 1) * R.amount), &lo);
+            *longest = max(first, last) - (int32_t)Forecast;
+        }
+        return (int32_t)n;
+    }
+};
+
+// packages of L rows, the last one shorter
+struct SubCut {
+    int32_t L;
+    __device__ int32_t operator()(int32_t n, int32_t* longest) const {
+        *longest = min(n, L);
+        return n / L + (n % L != 0);
+    }
+};
+
+// pieces of every series into cnt[s]; each kind's longest piece into info->kind_max_len (zeroed by the caller)
+template <class Cut>
+__global__ void k_piece_count(const int32_t* __restrict__ len, int64_t n_series, Cut cut, int n_kinds,
+                              int32_t* __restrict__ cnt, StackedInfo* info) {
     __shared__ int mx[TSFX_MAX_KINDS];
     for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) mx[k] = 0;
     __syncthreads();
     int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     for (; s < n_series; s += stride) {
-        const int32_t L = len[s];
-        int32_t t0, lo;
-        const int64_t n = roll_kept(R, L, &t0);
-        cnt[s] = (int32_t)n;
-        if (n > 0) {
-            const int32_t first = roll_window(R, L, t0, &lo);
-            const int32_t last = roll_window(R, L, (int32_t)(t0 + (n - 1) * R.amount), &lo);
-            atomicMax(&mx[kind_of_series(info, n_kinds, s)], max(first, last) - (int32_t)Forecast);
-        }
+        int32_t longest;
+        cnt[s] = cut(len[s], &longest);
+        if (longest > 0) atomicMax(&mx[kind_of_series(info, n_kinds, s)], longest);
     }
     __syncthreads();
     for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
@@ -693,97 +715,109 @@ __global__ void k_roll_kinds(const int32_t* __restrict__ off, int n_kinds, Stack
     for (int k = threadIdx.x; k <= n_kinds; k += blockDim.x) info->kind_series[k] = off[info->kind_series[k]];
 }
 
+// The working arrays of a regrouping (slots G_*): `bound` piece slots for the ns staged series
+struct Pieces {
+    int64_t ns, bound;
+    int32_t* off;                 // first piece of every series; off[ns] = the number of pieces
+    int64_t* begin;               // view of every piece on the staged values
+    int32_t* len;
+    int32_t* row;                 // union row of every piece
+    int64_t* id;                  // name of every piece: its parent id and a key
+    uint64_t* key;
+    int32_t* scan;                // the scanned name changes
+    size_t tb_off, tb_union;      // temporary storage of the two scans
+};
+
+static auto name_changes(const Pieces& P, const uint32_t* perm) {
+    return thrust::make_transform_iterator(thrust::counting_iterator<int64_t>(0), NameChange{P.id, P.key, perm, P.off + P.ns});
+}
+
+// Setup: the piece slots, the temporary storage of both scans, kind_max_len and off[ns] zeroed
+static int pieces_setup(StackedWorkspace& S, int64_t bound, Pieces* P, cudaStream_t st, std::string* msg) {
+    const int64_t ns = S.h_info->kind_series[S.n_kinds];
+    const size_t nb = (size_t)std::max<int64_t>(bound, 1);
+    CKE(S.reserve(G_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
+    CKE(S.reserve(G_BEGIN, nb * 8), "alloc pieces");
+    CKE(S.reserve(G_LEN, nb * 4), "alloc pieces");
+    CKE(S.reserve(G_ROW, nb * 4), "alloc pieces");
+    CKE(S.reserve(G_ID, nb * 8), "alloc pieces");
+    CKE(S.reserve(G_KEY, nb * 8), "alloc pieces");
+    CKE(S.reserve(G_SCAN, nb * 4), "alloc pieces");
+    CKE(S.reserve(G_UID, nb * 8), "alloc pieces");
+    CKE(S.reserve(G_UKEY, nb * 8), "alloc pieces");
+    *P = Pieces{ns, bound, (int32_t*)S.bufs[G_OFF], (int64_t*)S.bufs[G_BEGIN], (int32_t*)S.bufs[G_LEN], (int32_t*)S.bufs[G_ROW],
+                (int64_t*)S.bufs[G_ID], (uint64_t*)S.bufs[G_KEY], (int32_t*)S.bufs[G_SCAN], 0, 0};
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, P->tb_off, P->off, P->off, (int)(ns + 1), st), "scan size");
+    CKE(cub::DeviceScan::InclusiveSum(nullptr, P->tb_union, name_changes(*P, nullptr), P->scan, (int)bound, st), "scan size");
+    CKE(S.reserve(T_TEMP, std::max(P->tb_off, P->tb_union)), "alloc temp");
+    CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
+        "memset info");
+    CKE(cudaMemsetAsync(P->off + ns, 0, 4, st), "memset offsets");
+    return TSFX_OK;
+}
+
+// Offsets: the pieces of every series and each kind's longest piece, then the exclusive scan of the counts
+template <class Cut>
+static int pieces_count(StackedWorkspace& S, const Pieces& P, Cut cut, cudaStream_t st, std::string* msg) {
+    k_piece_count<<<grid_for(P.ns, 256), 256, 0, st>>>(S.d_len, P.ns, cut, S.n_kinds, P.off, S.d_info);
+    CKE(cudaGetLastError(), "piece count kernel");
+    size_t tb = P.tb_off;
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb, P.off, P.off, (int)(P.ns + 1), st), "piece offsets");
+    return TSFX_OK;
+}
+
+// Union: sort_rows over the names as (major, minor) pairs (minor float64 bits when minor_f64), the distinct names
+// flagged and scanned into the union row of every piece and the name (id, key) of every union row (S.d_uid / S.d_ukey);
+// each kind's series range becomes its piece range.  utarget (forecasting windows, with their targets): the target of
+// every union row.
+static int pieces_union(StackedWorkspace& S, CsrWorkspace& W, const Pieces& P, const int64_t* major, const uint64_t* minor,
+                        int minor_f64, const int64_t* target, int64_t* utarget, cudaStream_t st, std::string* msg) {
+    uint32_t* perm = nullptr;
+    if (int rc = sort_rows(W, major, minor, minor_f64, P.bound, st, msg, &perm)) return rc;
+    size_t tb = P.tb_union;
+    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb, name_changes(P, perm), P.scan, (int)P.bound, st), "union rows");
+    S.d_uid = (int64_t*)S.bufs[G_UID];
+    S.d_ukey = (uint64_t*)S.bufs[G_UKEY];
+    (utarget ? k_roll_union<true> : k_roll_union<false>)<<<grid_for(P.bound, 256), 256, 0, st>>>(
+        perm, P.scan, P.off + P.ns, P.id, P.key, P.row, S.d_uid, S.d_ukey, S.d_info, target, utarget);
+    k_roll_kinds<<<1, 128, 0, st>>>(P.off, S.n_kinds, S.d_info);
+    CKE(cudaGetLastError(), "union kernels");
+    return TSFX_OK;
+}
+
 int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction, int32_t max_timeshift, int32_t min_timeshift,
                  int32_t Lmax, int64_t bound, bool forecast, cudaStream_t st, std::string* msg) {
-    const int n_kinds = S.n_kinds;
-    const int64_t ns = S.h_info->kind_series[n_kinds];
     const int32_t given_min_ts = min_timeshift;
     if (forecast) min_timeshift = std::max(min_timeshift, 1);     // a window of one row is empty without its last row
     const RollSpec R = roll_spec(rolling_direction, max_timeshift, min_timeshift, Lmax);
-    const size_t nb = (size_t)std::max<int64_t>(bound, 1);
-    CKE(S.reserve(R_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
-    CKE(S.reserve(R_BEGIN, nb * 8), "alloc windows");
-    CKE(S.reserve(R_LEN, nb * 4), "alloc windows");
-    CKE(S.reserve(R_ROW, nb * 4), "alloc windows");
-    CKE(S.reserve(R_ID, nb * 8), "alloc windows");
-    CKE(S.reserve(R_KEY, nb * 8), "alloc windows");
-    CKE(S.reserve(R_SCAN, nb * 4), "alloc windows");
-    CKE(S.reserve(R_UID, nb * 8), "alloc windows");
-    CKE(S.reserve(R_UKEY, nb * 8), "alloc windows");
+    Pieces P;
+    if (int rc = pieces_setup(S, bound, &P, st, msg)) return rc;
+    int64_t *wtarget = nullptr, *utarget = nullptr;
     if (forecast) {
+        const size_t nb = (size_t)std::max<int64_t>(bound, 1);
         CKE(S.reserve(R_TGT, nb * 8), "alloc targets");
         CKE(S.reserve(R_UTGT, nb * 8), "alloc targets");
+        wtarget = (int64_t*)S.bufs[R_TGT];
+        utarget = (int64_t*)S.bufs[R_UTGT];
     }
-    int64_t* wtarget = forecast ? (int64_t*)S.bufs[R_TGT] : nullptr;
-    int64_t* utarget = forecast ? (int64_t*)S.bufs[R_UTGT] : nullptr;
-    int32_t* off = (int32_t*)S.bufs[R_OFF];
-    int64_t* wbegin = (int64_t*)S.bufs[R_BEGIN];
-    int32_t* wlen = (int32_t*)S.bufs[R_LEN];
-    int32_t* wrow = (int32_t*)S.bufs[R_ROW];
-    int64_t* wid = (int64_t*)S.bufs[R_ID];
-    uint64_t* wkey = (uint64_t*)S.bufs[R_KEY];
-    int32_t* scan = (int32_t*)S.bufs[R_SCAN];
     const int keys_f64 = S.d_keys && S.keys_f64;
-    uint32_t* perm = nullptr;
-    size_t tb1 = 0, tb2 = 0;
-    NameChange change{wid, wkey, nullptr, off + ns};
-    thrust::counting_iterator<int64_t> rows(0);
-    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb1, off, off, (int)(ns + 1), st), "scan size");
-    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st), "scan size");
-    CKE(S.reserve(T_TEMP, std::max(tb1, tb2)), "alloc temp");
-    // windows per series, their offsets, each kind's longest window
-    CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
-        "memset info");
-    CKE(cudaMemsetAsync(off + ns, 0, 4, st), "memset offsets");
-    (forecast ? k_roll_count<true> : k_roll_count<false>)<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, R, n_kinds, off,
-                                                                                               S.d_info);
-    CKE(cudaGetLastError(), "window count kernel");
-    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb1, off, off, (int)(ns + 1), st), "window offsets");
-    (forecast ? k_roll_fill<true> : k_roll_fill<false>)<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(
-        S.d_begin, S.d_len, S.d_row, S.d_uid, S.d_keys, keys_f64, off, ns, bound, R, wbegin, wlen, wid, wkey, S.d_info,
-        S.d_src, wtarget, given_min_ts);
+    if (int rc = forecast ? pieces_count(S, P, RollCut<true>{R}, st, msg) : pieces_count(S, P, RollCut<false>{R}, st, msg))
+        return rc;
+    (forecast ? k_roll_fill<true> : k_roll_fill<false>)<<<grid_for(std::max<int64_t>(P.ns * 32, bound), 256), 256, 0, st>>>(
+        S.d_begin, S.d_len, S.d_row, S.d_uid, S.d_keys, keys_f64, P.off, P.ns, bound, R, P.begin, P.len, P.id, P.key,
+        S.d_info, S.d_src, wtarget, given_min_ts);
     CKE(cudaGetLastError(), "window fill kernel");
-    // the union of the names: sort (id, name), flag and scan the distinct pairs
-    if (int rc = sort_rows(W, wid, wkey, keys_f64, bound, st, msg, &perm)) return rc;
-    change.perm = perm;
-    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st),
-        "union rows");
-    S.d_uid = (int64_t*)S.bufs[R_UID];
-    S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
-    (forecast ? k_roll_union<true> : k_roll_union<false>)<<<grid_for(bound, 256), 256, 0, st>>>(
-        perm, scan, off + ns, wid, wkey, wrow, S.d_uid, S.d_ukey, S.d_info, wtarget, utarget);
-    k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
-    CKE(cudaGetLastError(), "union kernels");
-    S.d_begin = wbegin;
-    S.d_len = wlen;
-    S.d_row = wrow;
+    // windows are named (parent id, key)
+    if (int rc = pieces_union(S, W, P, P.id, P.key, keys_f64, wtarget, utarget, st, msg)) return rc;
+    S.d_begin = P.begin;
+    S.d_len = P.len;
+    S.d_row = P.row;
     S.d_utarget = utarget;
-    S.rolled = true;
-    S.forecast = forecast;
-    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
-    return TSFX_OK;
+    return stacked_publish(S, st, msg);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // fixed-length packages of the staged series (stacked_sub)
-
-// packages of every series into cnt[s]; each kind's longest package (its longest series, cut at L) into
-// info->kind_max_len (zeroed by the caller)
-__global__ void k_sub_count(const int32_t* __restrict__ len, int64_t n_series, int32_t L, int n_kinds,
-                            int32_t* __restrict__ cnt, StackedInfo* info) {
-    __shared__ int mx[TSFX_MAX_KINDS];
-    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) mx[k] = 0;
-    __syncthreads();
-    int64_t s = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    for (; s < n_series; s += stride) {
-        const int32_t n = len[s];
-        cnt[s] = n / L + (n % L != 0);
-        if (n > 0) atomicMax(&mx[kind_of_series(info, n_kinds, s)], min(n, L));
-    }
-    __syncthreads();
-    for (int k = threadIdx.x; k < n_kinds; k += blockDim.x) if (mx[k]) atomicMax(&info->kind_max_len[k], mx[k]);
-}
 
 // Sort key of package slot i that puts every kind's packages in the order of their union rows: (kind, union row), or
 // INT64_MAX for the slots from *n_packages on.  Reads the kinds' package ranges (info->kind_series after k_roll_kinds).
@@ -840,72 +874,34 @@ __global__ void k_sub_fill(const int64_t* __restrict__ begin, const int32_t* __r
 }
 
 int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, cudaStream_t st, std::string* msg) {
-    const int n_kinds = S.n_kinds;
-    const int64_t ns = S.h_info->kind_series[n_kinds];
+    Pieces P;
+    if (int rc = pieces_setup(S, bound, &P, st, msg)) return rc;
     const size_t nb = (size_t)std::max<int64_t>(bound, 1);
-    CKE(S.reserve(R_OFF, (size_t)(ns + 1) * 4), "alloc offsets");
-    CKE(S.reserve(R_BEGIN, nb * 8), "alloc packages");
-    CKE(S.reserve(R_LEN, nb * 4), "alloc packages");
-    CKE(S.reserve(R_ROW, nb * 4), "alloc packages");
-    CKE(S.reserve(R_ID, nb * 8), "alloc packages");
-    CKE(S.reserve(R_KEY, nb * 8), "alloc packages");
-    CKE(S.reserve(R_SCAN, nb * 4), "alloc packages");
-    CKE(S.reserve(R_UID, nb * 8), "alloc packages");
-    CKE(S.reserve(R_UKEY, nb * 8), "alloc packages");
     CKE(S.reserve(P_BEGIN, nb * 8), "alloc packages");
     CKE(S.reserve(P_LEN, nb * 4), "alloc packages");
     CKE(S.reserve(P_ROW, nb * 4), "alloc packages");
-    int32_t* off = (int32_t*)S.bufs[R_OFF];
-    int64_t* pbegin = (int64_t*)S.bufs[R_BEGIN];
-    int32_t* plen = (int32_t*)S.bufs[R_LEN];
-    int32_t* prow = (int32_t*)S.bufs[R_ROW];
-    int64_t* pid = (int64_t*)S.bufs[R_ID];
-    int64_t* pnum = (int64_t*)S.bufs[R_KEY];
-    int32_t* scan = (int32_t*)S.bufs[R_SCAN];
-    uint32_t* perm = nullptr;
-    size_t tb1 = 0, tb2 = 0;
-    NameChange change{pid, (const uint64_t*)pnum, nullptr, off + ns};
-    thrust::counting_iterator<int64_t> rows(0);
-    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb1, off, off, (int)(ns + 1), st), "scan size");
-    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st), "scan size");
-    CKE(S.reserve(T_TEMP, std::max(tb1, tb2)), "alloc temp");
-    // packages per series, their offsets, each kind's longest package
-    CKE(cudaMemsetAsync((char*)S.d_info + offsetof(StackedInfo, kind_max_len), 0, sizeof(StackedInfo::kind_max_len), st),
-        "memset info");
-    CKE(cudaMemsetAsync(off + ns, 0, 4, st), "memset offsets");
-    k_sub_count<<<grid_for(ns, 256), 256, 0, st>>>(S.d_len, ns, L, n_kinds, off, S.d_info);
-    CKE(cudaGetLastError(), "package count kernel");
-    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb1, off, off, (int)(ns + 1), st), "package offsets");
-    k_sub_fill<<<grid_for(std::max<int64_t>(ns * 32, bound), 256), 256, 0, st>>>(S.d_begin, S.d_len, S.d_row, S.d_uid, off, ns,
-                                                                                 bound, L, pbegin, plen, pid, pnum);
+    if (int rc = pieces_count(S, P, SubCut{L}, st, msg)) return rc;
+    int64_t* pnum = (int64_t*)P.key;
+    k_sub_fill<<<grid_for(std::max<int64_t>(P.ns * 32, bound), 256), 256, 0, st>>>(S.d_begin, S.d_len, S.d_row, S.d_uid, P.off,
+                                                                                   P.ns, bound, L, P.begin, P.len, P.id, pnum);
     CKE(cudaGetLastError(), "package fill kernel");
-    // the union of the names: sort (package number, parent id), flag and scan the distinct pairs
-    if (int rc = sort_rows(W, pnum, (const uint64_t*)pid, 0, bound, st, msg, &perm)) return rc;
-    change.perm = perm;
-    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb2, thrust::make_transform_iterator(rows, change), scan, (int)bound, st),
-        "union rows");
-    S.d_uid = (int64_t*)S.bufs[R_UID];
-    S.d_ukey = (uint64_t*)S.bufs[R_UKEY];
-    k_roll_union<false><<<grid_for(bound, 256), 256, 0, st>>>(perm, scan, off + ns, pid, (const uint64_t*)pnum, prow, S.d_uid,
-                                                              S.d_ukey, S.d_info, nullptr, nullptr);
-    k_roll_kinds<<<1, 128, 0, st>>>(off, n_kinds, S.d_info);
-    CKE(cudaGetLastError(), "union kernels");
+    // packages are named (package number, parent id)
+    if (int rc = pieces_union(S, W, P, pnum, (const uint64_t*)P.id, 0, nullptr, nullptr, st, msg)) return rc;
     // The packages were filled series by series, (parent id, package number) order inside a kind, but the union rows
     // ascend in (package number, parent id).  Reorder every kind's packages by union row, so that a kind with a package
     // for every union row fills its columns in place, as tsfx_extract_staged expects.  The names are no longer needed:
     // the sort key goes into their storage.
     int64_t* key = pnum;
-    k_sub_layout_key<<<grid_for(bound, 256), 256, 0, st>>>(prow, off + ns, bound, n_kinds, S.d_info, key);
+    k_sub_layout_key<<<grid_for(bound, 256), 256, 0, st>>>(P.row, P.off + P.ns, bound, S.n_kinds, S.d_info, key);
     CKE(cudaGetLastError(), "package layout kernel");
+    uint32_t* perm = nullptr;
     if (int rc = sort_rows(W, key, nullptr, 0, bound, st, msg, &perm)) return rc;
     S.d_begin = (int64_t*)S.bufs[P_BEGIN];
     S.d_len = (int32_t*)S.bufs[P_LEN];
     S.d_row = (int32_t*)S.bufs[P_ROW];
-    k_sub_gather<<<grid_for(bound, 256), 256, 0, st>>>(perm, off + ns, pbegin, plen, prow, S.d_begin, S.d_len, S.d_row);
+    k_sub_gather<<<grid_for(bound, 256), 256, 0, st>>>(perm, P.off + P.ns, P.begin, P.len, P.row, S.d_begin, S.d_len, S.d_row);
     CKE(cudaGetLastError(), "package gather kernel");
-    S.packaged = true;
-    CKE(cudaMemcpyAsync(S.h_info, S.d_info, sizeof(StackedInfo), cudaMemcpyDeviceToHost, st), "D2H info");
-    return TSFX_OK;
+    return stacked_publish(S, st, msg);
 }
 
 __global__ void k_fill_nan(double* __restrict__ out, int64_t n_rows, int n_cols, int ld) {

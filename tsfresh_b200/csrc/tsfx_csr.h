@@ -102,6 +102,9 @@ struct StackedInfo {              // written by the device, read once by the hos
     int32_t kind_max_len[TSFX_MAX_KINDS];
 };
 
+// what the staged series are: the (kind, id) series of the staged rows, or what stacked_roll / stacked_sub replaced them by
+enum class Staged : uint8_t { Rows, Windows, ForecastWindows, Packages };
+
 struct StackedWorkspace {
     // the staged input: partitioned rows and per-series views (device), and what the host learnt about them
     float* d_values = nullptr;    // row values, kind-major, (id, sort key) order inside a kind
@@ -120,12 +123,11 @@ struct StackedWorkspace {
     StackedInfo* d_info = nullptr;
     int n_kinds = 0;
     int64_t n_union = 0;
-    bool valid = false;           // staged and not yet consumed
+    Staged staged = Staged::Rows;
+    bool pending = false;         // staged and not yet consumed by tsfx_extract_staged (staged outlives it: the row keys
+                                  // and targets stay readable)
     bool has_keys = false;        // the rows came with sort keys
     bool keys_f64 = false;        //   float64 ones
-    bool rolled = false;          // the staged series have been turned into windows (stacked_roll)
-    bool packaged = false;        // the staged series have been cut into packages (stacked_sub)
-    bool forecast = false;        // the windows are make_forecasting_frame's (stacked_roll with forecast)
     void* bufs[32] = {nullptr};
     size_t caps[32] = {0};
     cudaError_t reserve(int slot, size_t bytes);
@@ -157,11 +159,11 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
                  int32_t Lmax, int64_t bound, bool forecast, cudaStream_t st, std::string* msg);
 
 // Fixed-length packages (add_sub_time_series_index) of the staged series, as new staged series: package j of a series
-// of n rows is the view on its rows [j * L, min((j + 1) * L, n)), so each kind keeps its aligned rows.  Same structure as
-// stacked_roll (count, scan, fill with one warp per series, sort_rows over the names, flag and scan); a package is named
-// (package number, parent id) and the union rows ascend in that order.  d_uid / d_ukey get the parent id / package
-// number of every union row; d_info the package ranges of the kinds, their longest packages and n_union, copied to
-// h_info (the caller synchronises).  bound >= the number of packages.
+// of n rows is the view on its rows [j * L, min((j + 1) * L, n)), so each kind keeps its aligned rows.  The count, scan
+// and union are stacked_roll's (one code path for both), the fill is its own; a package is named (package number, parent
+// id) and the union rows ascend in that order, and one more sort puts every kind's packages in union-row order.  d_uid /
+// d_ukey get the parent id / package number of every union row; d_info the package ranges of the kinds, their longest
+// packages and n_union, copied to h_info (the caller synchronises).  bound >= the number of packages.
 int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, cudaStream_t st, std::string* msg);
 
 // out[r * ld + c] = NaN for r < n_rows, c < n_cols

@@ -438,8 +438,8 @@ def extract_features_rolled_device(ids, values, sort=None, kind=None, *, kinds=N
     roll_time_series's errors for its arguments before the device is touched, and ValueError for two windows of one kind
     with the same name (sort keys tied at their naming rows), NaN values or sort keys, kind codes out of range and windows
     longer than their kind's plan allows, before any feature kernel runs."""
-    roll = _roll_args(rolling_direction, max_timeshift, min_timeshift)
-    return _extract_staged(ids, values, sort, kind, kinds, None, roll, default_fc_parameters, kind_to_fc_parameters,
+    regroup = ("roll",) + _roll_args(rolling_direction, max_timeshift, min_timeshift)
+    return _extract_staged(ids, values, sort, kind, kinds, None, regroup, default_fc_parameters, kind_to_fc_parameters,
                            impute_function)[:4]
 
 
@@ -470,7 +470,7 @@ def extract_features_forecasting_device(x, kind, max_timeshift, rolling_directio
     longer than the plan allows, before any feature kernel runs.  The plan's length limits apply to the windows, not to
     the series."""
     import torch
-    roll = _roll_args(rolling_direction, max_timeshift, min_timeshift)
+    regroup = ("forecast",) + _roll_args(rolling_direction, max_timeshift, min_timeshift)
     for name, t in (("x", x), ("index", index)):
         if t is None and name == "index":
             continue
@@ -491,8 +491,8 @@ def extract_features_forecasting_device(x, kind, max_timeshift, rolling_directio
         raise ValueError("x must be a CUDA tensor, got one on %s" % x.device)
     if index is not None and index.device != x.device:
         raise ValueError("index is on %s, x on %s" % (index.device, x.device))
-    X, _, window_keys, columns, targets = _extract_staged(None, x, index, None, [kind], None, roll, default_fc_parameters,
-                                                          kind_to_fc_parameters, impute_function, forecast=True)
+    X, _, window_keys, columns, targets = _extract_staged(None, x, index, None, [kind], None, regroup,
+                                                          default_fc_parameters, kind_to_fc_parameters, impute_function)
     with torch.cuda.device(x.device):
         nan = torch.full((), float("nan"), dtype=x.dtype, device=x.device)
         y = torch.where(targets >= 0, x[targets.clamp(min=0)], nan)
@@ -532,22 +532,25 @@ def extract_features_sub_device(ids, values, sort=None, kind=None, *, kinds=None
     NaN values or sort keys, kind codes out of range and packages longer than their kind's plan allows, before any
     feature kernel runs."""
     L = _sub_length(sub_length)
-    X, package_ids, package_numbers, columns, _ = _extract_staged(ids, values, sort, kind, kinds, times, None,
+    X, package_ids, package_numbers, columns, _ = _extract_staged(ids, values, sort, kind, kinds, times, ("sub", L),
                                                                   default_fc_parameters, kind_to_fc_parameters,
-                                                                  impute_function, sub_length=L)
+                                                                  impute_function)
     return X, package_numbers, package_ids if ids is not None else None, columns
 
 
-def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_parameters, kind_to_fc_parameters,
-                    impute_function, sub_length=None, forecast=False):
-    """(X, row ids, row keys, columns, targets) of long-format rows, staged by kind and extracted; with roll =
-    (direction, max_timeshift, min_timeshift) the staged series are rolled into windows first (row keys: the windows'
-    naming keys), with sub_length they are cut into packages first (row keys: the package numbers; ids may then be
-    None), else row keys is None.  forecast (with roll; ids may then be None): the windows are make_forecasting_frame's
-    and targets holds the target input row of every window (-1: none), else targets is None."""
+def _extract_staged(ids, values, sort, kind, kinds, times, regroup, default_fc_parameters, kind_to_fc_parameters,
+                    impute_function):
+    """(X, row ids, row keys, columns, targets) of long-format rows, staged by kind and extracted.  regroup replaces the
+    staged series first: ("roll", direction, max_timeshift, min_timeshift) by their rolled windows (row keys: the
+    windows' naming keys), ("forecast", direction, max_timeshift, min_timeshift) by make_forecasting_frame's windows
+    (row keys as for "roll"; targets: the target input row of every window, -1: none; ids may be None), ("sub",
+    sub_length) by their packages (row keys: the package numbers; ids may be None).  regroup None: the series as
+    staged.  Row keys and targets are None where the regrouping has none."""
     import torch
-    n, kinds = _long_layout(ids, values, sort, kind, kinds, times, need_ids=sub_length is None and not forecast)
-    if roll is not None and n <= 1:
+    how = regroup[0] if regroup else None
+    windows, forecast = how in ("roll", "forecast"), how == "forecast"
+    n, kinds = _long_layout(ids, values, sort, kind, kinds, times, need_ids=how in (None, "roll"))
+    if windows and n <= 1:
         raise ValueError("Your time series container has zero or one rows!. Can not perform rolling.")
     default_fc_parameters = _default_settings(default_fc_parameters, kind_to_fc_parameters)
     plans = [_kind_plan(k, default_fc_parameters, kind_to_fc_parameters, has_datetime_index=times is not None)
@@ -574,18 +577,17 @@ def _extract_staged(ids, values, sort, kind, kinds, times, roll, default_fc_para
                 n_rows, rows, _ = ctx.stage_long_stacked(
                     i.data_ptr(), 0 if s is None else s.data_ptr(), s is not None and s.dtype == torch.float64,
                     v.data_ptr(), 0 if k is None else k.data_ptr(), k is not None and k.dtype == torch.int64, len(kinds),
-                    0 if t is None else t.data_ptr(), n, keep_sort_keys=roll is not None, keep_row_numbers=forecast)
-                if roll is not None:
-                    n_rows, _ = ctx.roll_staged(*roll, len(kinds), forecast=forecast)
-                    row_keys = torch.empty(n_rows, dtype=torch.int64 if s is None else s.dtype, device=dev)
+                    0 if t is None else t.data_ptr(), n, keep_sort_keys=windows, keep_row_numbers=forecast)
+                if how is not None:
+                    if windows:
+                        n_rows, _ = ctx.roll_staged(*regroup[1:], len(kinds), forecast=forecast)
+                    else:
+                        n_rows, _ = ctx.sub_staged(regroup[1], len(kinds))
+                    row_keys = torch.empty(n_rows, dtype=s.dtype if windows and s is not None else torch.int64, device=dev)
                     ctx.staged_row_keys(row_keys.data_ptr())
-                    if forecast:
-                        targets = torch.empty(n_rows, dtype=torch.int64, device=dev)
-                        ctx.staged_targets(targets.data_ptr())
-                elif sub_length is not None:
-                    n_rows, _ = ctx.sub_staged(sub_length, len(kinds))
-                    row_keys = torch.empty(n_rows, dtype=torch.int64, device=dev)
-                    ctx.staged_row_keys(row_keys.data_ptr())
+                if forecast:
+                    targets = torch.empty(n_rows, dtype=torch.int64, device=dev)
+                    ctx.staged_targets(targets.data_ptr())
                 present = [c for c in range(len(kinds)) if rows[c] > 0]
                 columns = [name for c in present for name in plans[c][1]]
                 width = len(columns)
