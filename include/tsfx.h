@@ -260,9 +260,46 @@ int tsfx_set_row_times(tsfx_ctx* ctx, const int64_t* row_time_ns, int64_t n_rows
 #define TSFX_STATUS_VIEW 2       /* first series with an invalid view */
 #define TSFX_STATUS_LONG 3       /* first valid series longer than max_len */
 #define TSFX_STATUS_NAN 4        /* first other series with a NaN value */
+#define TSFX_STATUS_KIND 5       /* tsfx_extract_long_deferred: 1 when a kind code is outside 0 .. n_kinds-1 */
+#define TSFX_STATUS_KEY_NAN 6    /* tsfx_extract_long_deferred: 1 when a float64 sort key is NaN */
+#define TSFX_STATUS_IDS 7        /* tsfx_extract_long_deferred: the number of distinct ids when it exceeds max_ids, else 0 */
+#define TSFX_STATUS_ID 2         /* tsfx_extract_long_deferred (whose slot views are never invalid): the id its report
+                                  * names -- the first id past max_ids, else the id of the first series longer than max_len,
+                                  * else -1 */
 #define TSFX_STATUS_WORDS 8
 int tsfx_prepare(tsfx_ctx* ctx, const tsfx_plan* plan, int64_t n_series, int32_t max_len);
 int tsfx_set_status(tsfx_ctx* ctx, int64_t* status);
+
+/* Deferred long format: tsfx_stage_long_stacked + tsfx_extract_staged in one call that only enqueues work, for a prepared
+ * shape, so that it overlaps other work and can be captured in a CUDA graph:
+ *   tsfx_prepare_long          plans[k] is kind k's plan (NULL: the kind has no columns), 1 <= n_kinds <= 64; the calls
+ *                              take at most max_rows rows (<= 2^31 - 4 098) with at most max_ids distinct ids and
+ *                              series of at most max_len samples (TSFX_E_TOO_LONG beyond a plan's limit).  Reserves every
+ *                              buffer of the stage for max_rows rows, the slot and check buffers of n_kinds x max_ids
+ *                              series, a staging block of max_ids x n_cols(k) doubles per kind, and calls tsfx_prepare for
+ *                              every plan with (max_ids, max_len).  Blocks.  The plans must outlive the calls; a later
+ *                              tsfx_prepare_long, tsfx_prepare or stage call on the context may move the working memory.
+ *   tsfx_extract_long_deferred n_rows device rows (ids, sort_keys, values, kind_codes as tsfx_stage_long_stacked takes them,
+ *                              TSFX_FLAG_DEVICE_PTRS required, no other flag), of which rows [0, *n_rows_live) count
+ *                              (n_rows_live: a device int64, clamped to 0 .. n_rows; NULL: all n_rows).  Fills out
+ *                              ([max_ids x ld] row-major float64, ld >= the total column count of all kinds, blocks in
+ *                              kind order): rows [0, *n_ids) are tsfx_extract_staged's rows for the live rows, every
+ *                              other cell NaN -- a kind without rows has NaN columns; out_ids (max_ids int64) gets the
+ *                              union ids ascending, then INT64_MAX; *n_ids (device int64) the union size.  Errors are
+ *                              the deferred input check's, reported to the tsfx_set_status words (required): a kind
+ *                              code out of range, a NaN float64 sort key or more than max_ids distinct ids reject the
+ *                              call (out all NaN, *n_ids 0, TSFX_STATUS_KIND / _KEY_NAN / _IDS); a NaN value, or more
+ *                              than max_len samples, in the series of one (id, kind) makes that series' cells NaN
+ *                              (TSFX_STATUS_NAN / _LONG: its slot k * max_ids + i, the i-th series of kind k in id
+ *                              order; TSFX_STATUS_ID: the id).  One call counts once in TSFX_STATUS_CALLS.  The call
+ *                              makes no allocation, no copy to the host and no synchronisation; a call that would need
+ *                              more than was prepared returns TSFX_E_INVALID (n_rows) or TSFX_E_CUDA before any work. */
+int tsfx_prepare_long(tsfx_ctx* ctx, const tsfx_plan* const* plans, int32_t n_kinds, int64_t max_rows, int64_t max_ids,
+                      int32_t max_len);
+int tsfx_extract_long_deferred(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
+                               const float* values, const void* kind_codes, int32_t kind_code_is_i64, int64_t n_rows,
+                               const int64_t* n_rows_live, int64_t* out_ids, int64_t* n_ids, double* out, int32_t ld,
+                               uint32_t flags);
 /* Longest series a plan of these columns accepts (TSFX_E_TOO_LONG beyond; 2^31 - 1 when no group limits it), or
  * TSFX_E_INVALID for an unknown calculator.  Needs no context or device. */
 int32_t tsfx_plan_max_len(const tsfx_feature_desc* descs, int32_t n_descs);

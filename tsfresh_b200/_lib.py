@@ -23,6 +23,7 @@ FLAG_KEEP_ROW_NUMBERS = 128
 FLAG_FORECAST = 256
 FLAG_DEFER_CHECK = 512
 STATUS_CALLS, STATUS_BAD, STATUS_VIEW, STATUS_LONG, STATUS_NAN, STATUS_WORDS = 0, 1, 2, 3, 4, 8
+STATUS_ID, STATUS_KIND, STATUS_KEY_NAN, STATUS_IDS = 2, 5, 6, 7          # tsfx_extract_long_deferred's report
 STREAM_LEGACY = 1                 # cudaStreamLegacy: the handle of the legacy default stream for tsfx_ctx_set_stream
 PEER_AUTO, PEER_COPY, PEER_STORE, PEER_MULTICAST = 0, 1, 2, 3
 IMPUTE_RANGE, IMPUTE_ZERO, IMPUTE_GIVEN, IMPUTE_STATS = 0, 1, 2, 3
@@ -44,7 +45,7 @@ EXPORTS = ["tsfx_ctx_create", "tsfx_ctx_destroy", "tsfx_last_error", "tsfx_sync"
            "tsfx_set_peer_outputs", "tsfx_peer_flush", "tsfx_set_max_len_hint", "tsfx_set_row_times", "tsfx_select_classification", "tsfx_extract_long_kinds", "tsfx_device_count", "tsfx_select_regression",
            "tsfx_ctx_set_stream", "tsfx_set_out_ld", "tsfx_stage_long_stacked", "tsfx_extract_staged",
            "tsfx_roll_staged", "tsfx_staged_row_keys", "tsfx_sub_staged", "tsfx_staged_targets",
-           "tsfx_prepare", "tsfx_set_status", "tsfx_plan_max_len"]
+           "tsfx_prepare", "tsfx_set_status", "tsfx_plan_max_len", "tsfx_prepare_long", "tsfx_extract_long_deferred"]
 
 
 def load():
@@ -103,6 +104,8 @@ def load():
         lib.tsfx_set_status.argtypes = [vp, vp]
         lib.tsfx_plan_max_len.argtypes = [vp, i32]
         lib.tsfx_plan_max_len.restype = i32
+        lib.tsfx_prepare_long.argtypes = [vp, vp, i32, i64, i64, i32]
+        lib.tsfx_extract_long_deferred.argtypes = [vp, vp, vp, i32, vp, vp, i32, i64, vp, vp, vp, vp, i32, u32]
         _lib = lib
         return lib
 
@@ -285,6 +288,22 @@ class Context:
         plans = (ctypes.c_void_p * len(device_plans))(*[None if dp is None else dp.h for dp in device_plans])
         rc = self.lib.tsfx_extract_staged(self.h, plans, ctypes.c_void_p(ids_ptr), ctypes.c_void_p(out_ptr), int(ld), flags)
         self.check(rc, "tsfx_extract_staged")
+
+    def prepare_long(self, device_plans, max_rows, max_ids, max_len):
+        """tsfx_prepare_long: device_plans[k] is kind k's DevicePlan (None: no columns).  Blocks."""
+        plans = (ctypes.c_void_p * len(device_plans))(*[None if dp is None else dp.h for dp in device_plans])
+        rc = self.lib.tsfx_prepare_long(self.h, plans, len(device_plans), int(max_rows), int(max_ids), int(max_len))
+        self.check(rc, "tsfx_prepare_long")
+
+    def extract_long_deferred(self, ids_ptr, sort_ptr, sort_is_f64, values_ptr, kind_ptr, kind_is_i64, n_rows, n_live_ptr,
+                              out_ids_ptr, n_ids_ptr, out_ptr, ld):
+        """tsfx_extract_long_deferred on device pointers (ints, 0 for an absent column or n_live): only enqueues"""
+        vp = ctypes.c_void_p
+        rc = self.lib.tsfx_extract_long_deferred(self.h, vp(ids_ptr or None), vp(sort_ptr or None), int(sort_is_f64),
+                                                 vp(values_ptr or None), vp(kind_ptr or None), int(kind_is_i64), int(n_rows),
+                                                 vp(n_live_ptr or None), vp(out_ids_ptr), vp(n_ids_ptr), vp(out_ptr or None),
+                                                 int(ld), FLAG_DEVICE_PTRS)
+        self.check(rc, "tsfx_extract_long_deferred")
 
     def impute_device(self, matrix_ptr, rows, cols, mode=IMPUTE_RANGE):
         rc = self.lib.tsfx_impute(self.h, ctypes.c_void_p(matrix_ptr), rows, cols, mode, None, FLAG_DEVICE_PTRS)

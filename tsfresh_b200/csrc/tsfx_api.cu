@@ -267,6 +267,12 @@ struct tsfx_ctx {
     int prep_len = 0;
     int64_t* status = nullptr;
     DevBuf defer;
+    // tsfx_prepare_long: the prepared long shape, its plans, its slot and check buffers and its per-kind staging blocks
+    int long_kinds = 0;
+    int64_t long_rows = 0, long_ids = 0;
+    int long_len = 0;
+    const tsfx_plan* long_plans[TSFX_MAX_KINDS];
+    DevBuf long_slots, long_out;
     HostPool pool;
     Stager stager;
     // multi-GPU result placement (tsfx_set_peer_outputs): peers' mapped result matrices
@@ -422,6 +428,7 @@ extern "C" void tsfx_ctx_destroy(tsfx_ctx* ctx) {
     ctx->values.release(); ctx->begin.release(); ctx->len.release(); ctx->out.release(); ctx->misc.release(); ctx->stage.release();
     ctx->times.release(); ctx->times_sorted.release(); ctx->kvals.release(); ctx->kvals_sorted.release();
     ctx->defer.release();
+    ctx->long_slots.release(); ctx->long_out.release();
     ctx->csr.release();
     ctx->stacked.release();
     ctx->imp.release();
@@ -1637,6 +1644,138 @@ extern "C" int tsfx_extract_staged(tsfx_ctx* ctx, const tsfx_plan* const* plans,
     CK(cudaMemcpyAsync(out_ids, S.d_uid, (size_t)U * sizeof(int64_t), cudaMemcpyDeviceToDevice, ctx->stream));
     ctx->launches = launched;
     if (flags & TSFX_FLAG_IMPUTE) return impute_after_extract(ctx, out, U, total);
+    return TSFX_OK;
+}
+
+// ------------------------------------------------------------------------------------------ deferred long format
+// tsfx_prepare_long's slot and check buffers for n = n_kinds x max_ids slots: per slot its view and union row
+// (stacked_slots), its private view and reject reason (defer_check); the first rejected slot per reason, the live
+// series of every kind and the first id past max_ids
+struct LongSlots {
+    unsigned long long* first;
+    int64_t *sbegin, *vbegin, *live, *id_past;
+    int32_t *slen, *vlen, *srow;
+    uint8_t* reject;
+};
+static size_t long_slot_bytes(int64_t n) { return 64 + 8 * (TSFX_MAX_KINDS + 1) + (size_t)n * 29; }
+static LongSlots long_slots(tsfx_ctx* ctx) {
+    char* p = (char*)ctx->long_slots.p;
+    const size_t n = (size_t)ctx->long_kinds * ctx->long_ids;
+    LongSlots B;
+    B.first = (unsigned long long*)p;
+    B.live = (int64_t*)(p + 64);
+    B.id_past = B.live + TSFX_MAX_KINDS;
+    p += 64 + 8 * (TSFX_MAX_KINDS + 1);
+    B.sbegin = (int64_t*)p;
+    B.vbegin = B.sbegin + n;
+    B.slen = (int32_t*)(B.vbegin + n);
+    B.vlen = B.slen + n;
+    B.srow = B.vlen + n;
+    B.reject = (uint8_t*)(B.srow + n);
+    return B;
+}
+
+extern "C" int tsfx_prepare_long(tsfx_ctx* ctx, const tsfx_plan* const* plans, int32_t n_kinds, int64_t max_rows, int64_t max_ids,
+                                 int32_t max_len) {
+    if (!ctx) return TSFX_E_INVALID;
+    if (n_kinds < 1 || n_kinds > TSFX_MAX_KINDS || !plans) return fail(ctx, TSFX_E_INVALID, "between 1 and 64 kinds per call");
+    if (max_rows < 1 || max_rows > kMaxStackedRows || max_ids < 1 || max_ids > 0x7fffffff || max_len < 1)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_prepare_long: max_rows in 1 .. 2^31 - 4 098, max_ids in 1 .. 2^31 - 1 and "
+                                         "max_len >= 1");
+    int64_t cols = 0;
+    for (int k = 0; k < n_kinds; ++k) {
+        if (plans[k] && plans[k]->ctx != ctx) return fail(ctx, TSFX_E_INVALID, "plan does not belong to this context");
+        if (plans[k]) cols += plans[k]->ncols;
+    }
+    CK(cudaSetDevice(ctx->device));
+    ctx->long_kinds = 0;                  // unprepared until every step succeeded
+    for (int k = 0; k < n_kinds; ++k) {
+        if (!plans[k] || plans[k]->ncols == 0) continue;
+        if (int rc = check_lengths(ctx, plans[k], max_len)) return rc;
+        if (int rc = reserve_groups(ctx, plans[k], max_ids, max_len)) return rc;
+    }
+    std::string msg;
+    ctx->stacked.frozen = ctx->csr.frozen = false;
+    if (int rc = stacked_defer_reserve(ctx->stacked, ctx->csr, max_rows, n_kinds, &msg)) return fail(ctx, rc, msg);
+    CK(ctx->long_slots.reserve(long_slot_bytes((int64_t)n_kinds * max_ids)));
+    CK(ctx->long_out.reserve(std::max<size_t>((size_t)max_ids * cols * sizeof(double), 8)));
+    for (int k = 0; k < n_kinds; ++k) ctx->long_plans[k] = plans[k] && plans[k]->ncols > 0 ? plans[k] : nullptr;
+    ctx->long_kinds = n_kinds;
+    ctx->long_rows = max_rows;
+    ctx->long_ids = max_ids;
+    ctx->long_len = max_len;
+    CK(cudaStreamSynchronize(ctx->stream));     // the tables are filled before a captured call, which cannot wait for them
+    return TSFX_OK;
+}
+
+// While a deferred call enqueues, the stage's workspaces fail instead of growing (a graph holds their addresses)
+struct FreezeStage {
+    tsfx_ctx* ctx;
+    explicit FreezeStage(tsfx_ctx* c) : ctx(c) { ctx->stacked.frozen = ctx->csr.frozen = true; }
+    ~FreezeStage() { ctx->stacked.frozen = ctx->csr.frozen = false; }
+};
+
+// stage -> slots -> deferred check -> every kind's groups on its slots -> report -> NaN matrix and scatter of the live
+// slots -> ids and status (tsfx.h "Deferred long format")
+extern "C" int tsfx_extract_long_deferred(tsfx_ctx* ctx, const int64_t* ids, const void* sort_keys, int32_t sort_key_is_f64,
+                                          const float* values, const void* kind_codes, int32_t kind_code_is_i64, int64_t n_rows,
+                                          const int64_t* n_rows_live, int64_t* out_ids, int64_t* n_ids, double* out, int32_t ld,
+                                          uint32_t flags) {
+    if (!ctx) return TSFX_E_INVALID;
+    ctx->launches = 0;
+    ctx->n_kernels = 0;
+    if (flags != TSFX_FLAG_DEVICE_PTRS) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred takes TSFX_FLAG_DEVICE_PTRS alone");
+    const int K = ctx->long_kinds;
+    const int64_t M = ctx->long_ids;
+    if (K == 0) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred: no shape prepared (tsfx_prepare_long)");
+    if (!ctx->status) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred needs a status buffer (tsfx_set_status)");
+    if (n_rows < 0 || n_rows > ctx->long_rows)
+        return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred: " + std::to_string(n_rows) + " rows, more than the " +
+                                             std::to_string(ctx->long_rows) + " tsfx_prepare_long made ready");
+    int col0[TSFX_MAX_KINDS], total = 0;
+    for (int k = 0; k < K; ++k) { col0[k] = total; if (ctx->long_plans[k]) total += ctx->long_plans[k]->ncols; }
+    if ((n_rows > 0 && (!ids || !values)) || !out_ids || !n_ids || (total > 0 && !out))
+        return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred: bad arguments");
+    if (ld < total) return fail(ctx, TSFX_E_INVALID, "tsfx_extract_long_deferred: row stride " + std::to_string(ld) + " < " +
+                                                       std::to_string(total) + " columns");
+    CK(cudaSetDevice(ctx->device));
+    StackedWorkspace& S = ctx->stacked;
+    FreezeStage freeze(ctx);
+    std::string msg;
+    // the sizes first, so that a call beyond the prepared buffers fails before it enqueues anything
+    if (int rc = stacked_defer_reserve(S, ctx->csr, std::max<int64_t>(n_rows, 1), K, &msg)) return fail(ctx, rc, msg);
+    const LongSlots B = long_slots(ctx);
+    const cudaStream_t st = ctx->stream;
+    CK(cudaMemsetAsync(B.first, 0, 3 * sizeof(unsigned long long), st));
+    if (int rc = stacked_stage_deferred(S, ctx->csr, ids, (const uint64_t*)sort_keys, sort_keys && sort_key_is_f64, values,
+                                        kind_codes, kind_code_is_i64, K, n_rows, n_rows_live, M, out_ids, B.id_past, st, &msg))
+        return fail(ctx, rc, msg);
+    CK(stacked_slots(S, K, M, B.sbegin, B.slen, B.srow, B.reject, B.live, st));
+    const int64_t n_pad = n_rows + (int64_t)K * TSFX_STACK_ALIGN;      // the staged values, alignment gaps included
+    CK(defer_check(S.d_values, n_pad, B.sbegin, B.slen, K * M, ctx->long_len, B.vbegin, B.vlen, B.reject, B.first, st, true));
+    int launched = 3;
+    double* block = (double*)ctx->long_out.p;
+    for (int k = 0; k < K; ++k) {
+        const tsfx_plan* P = ctx->long_plans[k];
+        if (!P) continue;
+        SeriesRef R;
+        R.values = S.d_values; R.begin = B.vbegin + k * M; R.len = B.vlen + k * M; R.dense_len = 0; R.n_series = M;
+        R.times = nullptr;
+        if (int rc = run_groups(ctx, P, R, ctx->long_len, block + M * col0[k], 0, P->ncols)) return rc;
+        launched += ctx->launches;
+    }
+    // the report only (no columns: the rejected slots are left out of the scatter, so their cells keep the NaN fill)
+    CK(defer_finish(nullptr, K * M, 0, 0, B.reject, B.first, ctx->status, st));
+    CK(stacked_fill_nan(out, M, total, ld, st));
+    launched += 2;
+    for (int k = 0; k < K; ++k) {
+        const tsfx_plan* P = ctx->long_plans[k];
+        if (!P) continue;
+        CK(stacked_scatter(block + M * col0[k], M, P->ncols, B.srow + k * M, out + col0[k], ld, st, B.live + k, B.reject + k * M));
+        launched += 1;
+    }
+    CK(stacked_defer_report(S, M, B.id_past, B.srow, out_ids, n_ids, ctx->status, st));
+    ctx->launches = launched + 1;
     return TSFX_OK;
 }
 

@@ -15,6 +15,7 @@ enum { S_IDS = 0, S_KEYS, S_VALS, S_PERM_A, S_PERM_B, S_KEY_A, S_KEY_B, S_TEMP, 
 
 cudaError_t CsrWorkspace::reserve(int slot, size_t bytes) {
     if (bytes <= caps[slot]) return cudaSuccess;
+    if (frozen) return cudaErrorMemoryAllocation;
     if (bufs[slot]) cudaFree(bufs[slot]);
     bufs[slot] = nullptr;
     caps[slot] = 0;
@@ -232,19 +233,28 @@ void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, c
 
 // Stable sort of the row index by (id, sort key) (sort key nullptr: by id alone): *perm_out = input row of every sorted
 // row, and S_KEY_B holds the sorted ids as ordered keys (key_i64).
-static int sort_rows(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, int64_t n, cudaStream_t st,
-                     std::string* msg, uint32_t** perm_out_) {
-    const int threads = 256;
-    const int blocks = grid_for(n, threads);
+// the buffers of sort_rows over n rows; *tb = the radix sort's temporary storage
+static int sort_reserve(CsrWorkspace& W, int64_t n, size_t* tb, cudaStream_t st, std::string* msg) {
     CKE(W.reserve(S_PERM_A, n * 4), "alloc perm");
     CKE(W.reserve(S_PERM_B, n * 4), "alloc perm");
     CKE(W.reserve(S_KEY_A, n * 8), "alloc key");
     CKE(W.reserve(S_KEY_B, n * 8), "alloc key");
     uint32_t *pa = (uint32_t*)W.bufs[S_PERM_A], *pb = (uint32_t*)W.bufs[S_PERM_B];
     uint64_t *ka = (uint64_t*)W.bufs[S_KEY_A], *kb = (uint64_t*)W.bufs[S_KEY_B];
+    *tb = 0;
+    CKE(cub::DeviceRadixSort::SortPairs(nullptr, *tb, ka, kb, pa, pb, (int)n, 0, 64, st), "radix size");
+    CKE(W.reserve(S_TEMP, *tb), "alloc temp");
+    return TSFX_OK;
+}
+
+static int sort_rows(CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int is_f64, int64_t n, cudaStream_t st,
+                     std::string* msg, uint32_t** perm_out_) {
+    const int threads = 256;
+    const int blocks = grid_for(n, threads);
     size_t tb = 0;
-    CKE(cub::DeviceRadixSort::SortPairs(nullptr, tb, ka, kb, pa, pb, (int)n, 0, 64, st), "radix size");
-    CKE(W.reserve(S_TEMP, tb), "alloc temp");
+    if (int rc = sort_reserve(W, n, &tb, st, msg)) return rc;
+    uint32_t *pa = (uint32_t*)W.bufs[S_PERM_A], *pb = (uint32_t*)W.bufs[S_PERM_B];
+    uint64_t *ka = (uint64_t*)W.bufs[S_KEY_A], *kb = (uint64_t*)W.bufs[S_KEY_B];
     const uint32_t* perm = pa;
     k_make_keys<<<blocks, threads, 0, st>>>(d_keys, is_f64, n, d_keys ? ka : nullptr, pa);
     if (d_keys) {      // pass A: stable sort of row indices by sort key
@@ -294,6 +304,7 @@ static_assert(T_SLOTS <= 32, "StackedWorkspace::bufs");
 
 cudaError_t StackedWorkspace::reserve(int slot, size_t bytes) {
     if (bytes <= caps[slot]) return cudaSuccess;
+    if (frozen) return cudaErrorMemoryAllocation;
     if (bufs[slot]) cudaFree(bufs[slot]);
     bufs[slot] = nullptr;
     caps[slot] = 0;
@@ -327,23 +338,27 @@ static int stacked_publish(StackedWorkspace& S, cudaStream_t st, std::string* ms
 #define STACK_NO_KIND 0xFFu
 
 // Counting-sort histogram over the rows in CSR order: kind code of every row (STACK_NO_KIND when out of range), rows per
-// (kind, tile) into counts[k * n_tiles + tile]; NaN float64 sort keys (input order) are flagged on the way.
+// (kind, tile) into counts[k * n_tiles + tile]; NaN float64 sort keys (input order) are flagged on the way.  n_live
+// (deferred stage; nullptr: every row counts): input rows from *n_live on are STACK_NO_KIND too, without a flag.
 __global__ void __launch_bounds__(STACK_THREADS) k_stack_count(const uint32_t* __restrict__ perm, const void* kinds, int kinds_i64,
                                                                int n_kinds, const uint64_t* __restrict__ keys_f64, int64_t n,
-                                                               uint8_t* __restrict__ code, int* __restrict__ counts, StackedInfo* info) {
+                                                               uint8_t* __restrict__ code, int* __restrict__ counts, StackedInfo* info,
+                                                               const int64_t* __restrict__ n_live) {
     __shared__ int hist[TSFX_MAX_KINDS];
     for (int k = threadIdx.x; k < TSFX_MAX_KINDS; k += blockDim.x) hist[k] = 0;
     __syncthreads();
     const int64_t lo = (int64_t)blockIdx.x * STACK_TILE, hi = min(lo + STACK_TILE, n);
+    const int64_t live = n_live ? *n_live : n;
     int bad = 0, nan = 0;
     for (int64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
         const uint32_t src = perm[i];
+        const bool dropped = (int64_t)src >= live;
         int64_t c = 0;
-        if (kinds) c = kinds_i64 ? ((const int64_t*)kinds)[src] : (int64_t)((const int32_t*)kinds)[src];
-        const bool ok = c >= 0 && c < n_kinds;
+        if (kinds && !dropped) c = kinds_i64 ? ((const int64_t*)kinds)[src] : (int64_t)((const int32_t*)kinds)[src];
+        const bool ok = !dropped && c >= 0 && c < n_kinds;
         code[i] = ok ? (uint8_t)c : (uint8_t)STACK_NO_KIND;
         if (ok) atomicAdd(&hist[c], 1);
-        bad |= !ok;
+        bad |= !ok && !dropped;
         if (keys_f64) { const double v = __longlong_as_double((long long)keys_f64[i]); nan |= v != v; }
     }
     if (__any_sync(0xffffffffu, bad) && (threadIdx.x & 31) == 0) atomicOr(&info->bad_kind, 1);
@@ -475,19 +490,18 @@ __global__ void k_stack_finish(const CsrInfo* csr, StackedInfo* info) {
     info->nan_values = csr->has_nan;
 }
 
-int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
-                  const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
-                  int64_t n, bool keep_keys, bool keep_rows, cudaStream_t st, std::string* msg) {
-    S.n_kinds = n_kinds;
-    S.has_keys = d_keys != nullptr;
-    S.keys_f64 = d_keys && keys_f64;
-    if (!S.h_info) CKE(cudaHostAlloc((void**)&S.h_info, sizeof(StackedInfo), cudaHostAllocDefault), "alloc info");
+// the device info of a stage, zeroed
+static int stack_info(StackedWorkspace& S, cudaStream_t st, std::string* msg) {
     CKE(S.reserve(T_INFO, sizeof(StackedInfo)), "alloc info");
     S.d_info = (StackedInfo*)S.bufs[T_INFO];
     CKE(cudaMemsetAsync(S.d_info, 0, sizeof(StackedInfo), st), "memset info");
-    // stage (a) over every row: (id, sort key) order, union of the ids, NaN scan of the values
-    int rc = csr_sort_pass(W, d_ids, d_keys, keys_f64, d_values, n, n, 1, true, st, msg);
-    if (rc) return rc;
+    return TSFX_OK;
+}
+
+// The partition's buffers for n rows of n_kinds kinds (row times, kept sort keys and row numbers when asked for) and the
+// temporary storage of its three scans (sizes into tb[3]; the scans read the sorted ids at ids_sorted)
+static int stack_reserve(StackedWorkspace& S, int64_t n, int n_kinds, bool times, bool keep_keys, bool keep_rows,
+                         const int64_t* ids_sorted, size_t* tb, cudaStream_t st, std::string* msg) {
     const int n_tiles = (int)((n + STACK_TILE - 1) / STACK_TILE);
     const int64_t n_pad = n + (int64_t)n_kinds * TSFX_STACK_ALIGN;       // partitioned rows and alignment gaps
     const size_t n_counts = (size_t)n_kinds * n_tiles + 1;
@@ -499,10 +513,58 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     CKE(S.reserve(T_BEGIN, (size_t)n * 8), "alloc begin");
     CKE(S.reserve(T_LEN, (size_t)n * 4), "alloc len");
     CKE(S.reserve(T_ROW, (size_t)n * 4), "alloc map");
-    if (d_times) CKE(S.reserve(T_TIMES, (size_t)n_pad * 8), "alloc times");
-    keep_keys = keep_keys && d_keys;
+    if (times) CKE(S.reserve(T_TIMES, (size_t)n_pad * 8), "alloc times");
     if (keep_keys) CKE(S.reserve(T_KEYS, (size_t)n_pad * 8), "alloc keys");
     if (keep_rows) CKE(S.reserve(T_SRC, (size_t)n_pad * 4), "alloc row numbers");
+    int32_t* urow = (int32_t*)S.bufs[T_UROW];
+    int* counts = (int*)S.bufs[T_COUNTS];
+    thrust::counting_iterator<int64_t> rows(0);
+    auto id_change = thrust::make_transform_iterator(rows, IdChange{ids_sorted});
+    auto series_start = thrust::make_transform_iterator(rows, SeriesStart{(int32_t*)S.bufs[T_SROW], S.d_info, n_kinds});
+    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb[0], id_change, urow, (int)n, st), "scan size");
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb[1], counts, counts, (int)n_counts, st), "scan size");
+    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb[2], series_start, urow, (int)(n_pad + 1), st), "scan size");
+    CKE(S.reserve(T_TEMP, std::max(tb[0], std::max(tb[1], tb[2]))), "alloc temp");
+    return TSFX_OK;
+}
+
+// Deferred stage: the union size, union ids below max_ids and first id past them (stacked_stage_deferred)
+struct DeferredUnion {
+    const int64_t* n_live;
+    int64_t max_ids;
+    int64_t* out_ids;
+    int64_t* id_past;
+};
+
+// Union rows of the live rows [0, *n_live) of the sorted ids (the dropped rows sort after them): the union size into
+// info->n_union, the id of union row u into out_ids[u] below max_ids, the id of union row max_ids into *id_past
+__global__ void k_defer_union(const int32_t* __restrict__ urow, const int64_t* __restrict__ ids_sorted, int64_t n,
+                              DeferredUnion U, StackedInfo* info) {
+    const int64_t live = U.n_live ? max((int64_t)0, min(*U.n_live, n)) : n;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    if (i == 0) info->n_union = live > 0 ? (int64_t)urow[live - 1] + 1 : 0;
+    for (; i < live; i += stride)
+        if (i == 0 || urow[i] != urow[i - 1]) {
+            const int64_t u = urow[i];
+            if (u < U.max_ids) U.out_ids[u] = ids_sorted[i];
+            else if (u == U.max_ids) *U.id_past = ids_sorted[i];
+        }
+}
+
+// The sorted rows (W.d_perm, W.d_values, W's sorted ids) partitioned by kind: union rows, the kind counting sort, the
+// series' views, union rows and lengths (tsfx_csr.h).  D (deferred stage; nullptr: stacked_stage): the rows from
+// *D->n_live on are dropped, and the union is taken from the live rows.
+static int stack_partition(StackedWorkspace& S, CsrWorkspace& W, const uint64_t* d_keys, int keys_f64, const void* d_kinds,
+                           int kinds_i64, int n_kinds, const int64_t* d_times, int64_t n, bool keep_keys, bool keep_rows,
+                           const DeferredUnion* D, cudaStream_t st, std::string* msg) {
+    const int n_tiles = (int)((n + STACK_TILE - 1) / STACK_TILE);
+    const int64_t n_pad = n + (int64_t)n_kinds * TSFX_STACK_ALIGN;       // partitioned rows and alignment gaps
+    const size_t n_counts = (size_t)n_kinds * n_tiles + 1;
+    keep_keys = keep_keys && d_keys;
+    const int64_t* ids_sorted = (const int64_t*)W.bufs[S_IDS_SORTED];
+    size_t tb[3] = {0, 0, 0};
+    if (int rc = stack_reserve(S, n, n_kinds, d_times != nullptr, keep_keys, keep_rows, ids_sorted, tb, st, msg)) return rc;
     uint8_t* code = (uint8_t*)S.bufs[T_CODE];
     int32_t* urow = (int32_t*)S.bufs[T_UROW];      // union row of every CSR row; later the series index of every staged row
     int* counts = (int*)S.bufs[T_COUNTS];
@@ -514,34 +576,180 @@ int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, co
     S.d_begin = (int64_t*)S.bufs[T_BEGIN];
     S.d_len = (int32_t*)S.bufs[T_LEN];
     S.d_row = (int32_t*)S.bufs[T_ROW];
-    const int64_t* ids_sorted = (const int64_t*)W.bufs[S_IDS_SORTED];
     thrust::counting_iterator<int64_t> rows(0);
-    size_t tb1 = 0, tb2 = 0, tb3 = 0;
     auto id_change = thrust::make_transform_iterator(rows, IdChange{ids_sorted});
     SeriesStart start{srow, S.d_info, n_kinds};
     auto series_start = thrust::make_transform_iterator(rows, start);
-    CKE(cub::DeviceScan::InclusiveSum(nullptr, tb1, id_change, urow, (int)n, st), "scan size");
-    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb2, counts, counts, (int)n_counts, st), "scan size");
-    CKE(cub::DeviceScan::ExclusiveSum(nullptr, tb3, series_start, urow, (int)(n_pad + 1), st), "scan size");
-    const size_t tb = std::max(tb1, std::max(tb2, tb3));
-    CKE(S.reserve(T_TEMP, tb), "alloc temp");
-    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb1, id_change, urow, (int)n, st), "union rows");
+    CKE(cub::DeviceScan::InclusiveSum(S.bufs[T_TEMP], tb[0], id_change, urow, (int)n, st), "union rows");
+    if (D) {
+        k_defer_union<<<grid_for(n, 256), 256, 0, st>>>(urow, ids_sorted, n, *D, S.d_info);
+        CKE(cudaGetLastError(), "union kernel");
+    }
     k_stack_count<<<n_tiles, STACK_THREADS, 0, st>>>(W.d_perm, d_kinds, kinds_i64, n_kinds, keys_f64 ? d_keys : nullptr, n,
-                                                     code, counts, S.d_info);
+                                                     code, counts, S.d_info, D ? D->n_live : nullptr);
     CKE(cudaGetLastError(), "kind count kernel");
     CKE(cudaMemsetAsync(counts + n_counts - 1, 0, 4, st), "memset counts");
-    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb2, counts, counts, (int)n_counts, st), "kind offsets");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb[1], counts, counts, (int)n_counts, st), "kind offsets");
     k_stack_kind_rows<<<1, 1, 0, st>>>(counts, n_kinds, n_tiles, S.d_info);
     k_stack_scatter<<<n_tiles, STACK_THREADS, 0, st>>>(code, counts, n_kinds, n, W.d_values, urow, d_times,
                                                        keep_keys ? d_keys : nullptr, W.d_perm, S.d_info, S.d_values, srow,
                                                        S.d_times, S.d_keys, S.d_src);
     CKE(cudaGetLastError(), "kind scatter kernel");
-    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb3, series_start, urow, (int)(n_pad + 1), st), "series index");
+    CKE(cub::DeviceScan::ExclusiveSum(S.bufs[T_TEMP], tb[2], series_start, urow, (int)(n_pad + 1), st), "series index");
     k_stack_series<<<grid_for(n_pad, 256), 256, 0, st>>>(urow, start, n_pad, S.d_begin, S.d_row);
     k_stack_lengths<<<grid_for(n / 4 + 1, 256), 256, 0, st>>>(urow, n_pad, n_kinds, S.d_begin, S.d_len, S.d_info);
+    CKE(cudaGetLastError(), "series kernels");
+    return TSFX_OK;
+}
+
+int stacked_stage(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
+                  const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, const int64_t* d_times,
+                  int64_t n, bool keep_keys, bool keep_rows, cudaStream_t st, std::string* msg) {
+    S.n_kinds = n_kinds;
+    S.has_keys = d_keys != nullptr;
+    S.keys_f64 = d_keys && keys_f64;
+    if (!S.h_info) CKE(cudaHostAlloc((void**)&S.h_info, sizeof(StackedInfo), cudaHostAllocDefault), "alloc info");
+    if (int rc = stack_info(S, st, msg)) return rc;
+    // stage (a) over every row: (id, sort key) order, union of the ids, NaN scan of the values
+    int rc = csr_sort_pass(W, d_ids, d_keys, keys_f64, d_values, n, n, 1, true, st, msg);
+    if (rc) return rc;
+    rc = stack_partition(S, W, d_keys, keys_f64, d_kinds, kinds_i64, n_kinds, d_times, n, keep_keys, keep_rows, nullptr, st, msg);
+    if (rc) return rc;
     k_stack_finish<<<1, 1, 0, st>>>(W.d_info, S.d_info);
     CKE(cudaGetLastError(), "series kernels");
     return stacked_publish(S, st, msg);
+}
+
+// Deferred stage: the id and sort-key columns with the rows from *n_live on made to sort after every live row: id
+// INT64_MAX and the largest key that is not NaN (int64 INT64_MAX, float64 +inf), so the stable sorts keep them behind the
+// live rows with the same id and key.  A live NaN key rejects the call, so its place does not matter.
+__global__ void k_defer_rows(const int64_t* __restrict__ ids, const uint64_t* __restrict__ keys, int keys_f64, int64_t n,
+                             const int64_t* __restrict__ n_live, int64_t* __restrict__ ids_out, uint64_t* __restrict__ keys_out) {
+    const int64_t live = n_live ? *n_live : n;
+    const uint64_t last_key = keys_f64 ? 0x7ff0000000000000ull : 0x7fffffffffffffffull;
+    int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; i < n; i += stride) {
+        const bool dropped = i >= live;
+        ids_out[i] = dropped ? INT64_MAX : ids[i];
+        if (keys) keys_out[i] = dropped ? last_key : keys[i];
+    }
+}
+
+int stacked_defer_reserve(StackedWorkspace& S, CsrWorkspace& W, int64_t n, int n_kinds, std::string* msg) {
+    cudaStream_t st = 0;          // size queries only
+    CKE(W.reserve(S_IDS, (size_t)n * 8), "alloc ids");
+    CKE(W.reserve(S_KEYS, (size_t)n * 8), "alloc keys");
+    CKE(W.reserve(S_IDS_SORTED, (size_t)n * 8), "alloc ids sorted");
+    size_t tb = 0;
+    if (int rc = sort_reserve(W, n, &tb, st, msg)) return rc;
+    CKE(S.reserve(T_INFO, sizeof(StackedInfo)), "alloc info");
+    S.d_info = (StackedInfo*)S.bufs[T_INFO];
+    size_t tbs[3] = {0, 0, 0};
+    return stack_reserve(S, n, n_kinds, false, false, false, (const int64_t*)W.bufs[S_IDS_SORTED], tbs, st, msg);
+}
+
+int stacked_stage_deferred(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
+                           const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, int64_t n,
+                           const int64_t* d_n_live, int64_t max_ids, int64_t* out_ids, int64_t* id_past, cudaStream_t st,
+                           std::string* msg) {
+    S.n_kinds = n_kinds;
+    S.has_keys = d_keys != nullptr;
+    S.keys_f64 = d_keys && keys_f64;
+    S.d_times = nullptr;
+    S.d_keys = nullptr;
+    S.d_src = nullptr;
+    S.staged = Staged::Rows;
+    S.pending = false;
+    if (int rc = stack_info(S, st, msg)) return rc;
+    if (n == 0) {                         // the zeroed info: no union row, no series (the slots still view the values)
+        S.d_values = (float*)S.bufs[T_VALS];
+        S.d_begin = (int64_t*)S.bufs[T_BEGIN];
+        S.d_len = (int32_t*)S.bufs[T_LEN];
+        S.d_row = (int32_t*)S.bufs[T_ROW];
+        return TSFX_OK;
+    }
+    CKE(W.reserve(S_IDS, (size_t)n * 8), "alloc ids");
+    if (d_keys) CKE(W.reserve(S_KEYS, (size_t)n * 8), "alloc keys");
+    CKE(W.reserve(S_IDS_SORTED, (size_t)n * 8), "alloc ids sorted");
+    k_defer_rows<<<grid_for(n, 256), 256, 0, st>>>(d_ids, d_keys, keys_f64, n, d_n_live, W.ids(), W.keys());
+    CKE(cudaGetLastError(), "row kernel");
+    const uint64_t* keys = d_keys ? W.keys() : nullptr;
+    uint32_t* perm = nullptr;
+    if (int rc = sort_rows(W, W.ids(), keys, keys_f64, n, st, msg, &perm)) return rc;
+    uint64_t *ka = (uint64_t*)W.bufs[S_KEY_A], *kb = (uint64_t*)W.bufs[S_KEY_B];
+    k_gather_final<<<grid_for(n, 256), 256, 0, st>>>(kb, d_values, perm, n, (int64_t*)W.bufs[S_IDS_SORTED], (float*)ka);
+    CKE(cudaGetLastError(), "gather kernel");
+    W.d_values = (float*)ka;
+    W.d_perm = perm;
+    const DeferredUnion D{d_n_live, max_ids, out_ids, id_past};
+    return stack_partition(S, W, keys, keys_f64, d_kinds, kinds_i64, n_kinds, nullptr, n, false, false, &D, st, msg);
+}
+
+// kind k's series into the slots [k * max_ids, (k + 1) * max_ids) (stacked_slots)
+__global__ void k_defer_slots(const int64_t* __restrict__ begin, const int32_t* __restrict__ len, const int32_t* __restrict__ row,
+                              const StackedInfo* info, int n_kinds, int64_t max_ids, int64_t* __restrict__ sbegin,
+                              int32_t* __restrict__ slen, int32_t* __restrict__ srow, uint8_t* __restrict__ reject,
+                              int64_t* __restrict__ live) {
+    const bool whole = info->bad_kind || info->nan_keys || info->n_union > max_ids;
+    int64_t j = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (; j < (int64_t)n_kinds * max_ids; j += stride) {
+        const int k = (int)(j / max_ids);
+        const int64_t i = j - (int64_t)k * max_ids;
+        const int64_t s0 = info->kind_series[k];
+        const int64_t ns = whole ? 0 : info->kind_series[k + 1] - s0;        // <= n_union <= max_ids
+        if (i < ns) {
+            sbegin[j] = begin[s0 + i];
+            slen[j] = len[s0 + i];
+            srow[j] = row[s0 + i];
+            reject[j] = 0;
+        } else {
+            sbegin[j] = 0;
+            slen[j] = 1;
+            srow[j] = 0;
+            reject[j] = DEFER_UNUSED;
+        }
+        if (i == 0) live[k] = ns;
+    }
+}
+
+cudaError_t stacked_slots(const StackedWorkspace& S, int n_kinds, int64_t max_ids, int64_t* sbegin, int32_t* slen,
+                          int32_t* srow, uint8_t* reject, int64_t* live, cudaStream_t st) {
+    k_defer_slots<<<grid_for((int64_t)n_kinds * max_ids, 256), 256, 0, st>>>(S.d_begin, S.d_len, S.d_row, S.d_info, n_kinds,
+                                                                             max_ids, sbegin, slen, srow, reject, live);
+    return cudaGetLastError();
+}
+
+__global__ void k_defer_report(const StackedInfo* info, int64_t max_ids, const int64_t* __restrict__ id_past,
+                               const int32_t* __restrict__ srow, int64_t* __restrict__ out_ids, int64_t* n_ids, int64_t* status) {
+    const bool over = info->n_union > max_ids;
+    const bool whole = info->bad_kind || info->nan_keys || over;
+    const int64_t U = whole ? 0 : info->n_union;
+    int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u == 0) {                         // one thread: the calls on a status buffer are stream-ordered
+        *n_ids = U;
+        const int64_t call = status[TSFX_STATUS_CALLS];       // counted by k_defer_finish
+        if (whole && status[TSFX_STATUS_BAD] == 0) {
+            status[TSFX_STATUS_BAD] = call;
+            for (int r = 0; r < 3; ++r) status[TSFX_STATUS_VIEW + r] = -1;
+        }
+        if (status[TSFX_STATUS_BAD] == call) {
+            status[TSFX_STATUS_KIND] = info->bad_kind != 0;
+            status[TSFX_STATUS_KEY_NAN] = info->nan_keys != 0;
+            status[TSFX_STATUS_IDS] = over ? info->n_union : 0;
+            const int64_t s = status[TSFX_STATUS_LONG];
+            status[TSFX_STATUS_ID] = over ? *id_past : (!whole && s >= 0) ? out_ids[srow[s]] : -1;
+        }
+    }
+    for (const int64_t stride = (int64_t)gridDim.x * blockDim.x; u < max_ids; u += stride)
+        if (u >= U) out_ids[u] = INT64_MAX;
+}
+
+cudaError_t stacked_defer_report(const StackedWorkspace& S, int64_t max_ids, const int64_t* id_past, const int32_t* srow,
+                                 int64_t* out_ids, int64_t* n_ids, int64_t* status, cudaStream_t st) {
+    k_defer_report<<<grid_for(max_ids, 256), 256, 0, st>>>(S.d_info, max_ids, id_past, srow, out_ids, n_ids, status);
+    return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -917,11 +1125,14 @@ cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cu
 }
 
 __global__ void k_scatter_rows(const double* __restrict__ block, int64_t n_series, int n_cols, const int32_t* __restrict__ row,
-                               double* __restrict__ out, int ld) {
+                               double* __restrict__ out, int ld, const int64_t* __restrict__ count,
+                               const uint8_t* __restrict__ skip) {
     const int lane = threadIdx.x & 31;
     int64_t s = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    if (count) n_series = min(n_series, *count);
     for (; s < n_series; s += n_warps) {
+        if (skip && skip[s]) continue;    // warp-uniform
         const double* src = block + (size_t)s * n_cols;
         double* dst = out + (size_t)row[s] * ld;
         for (int c = lane; c < n_cols; c += 32) __stcs(dst + c, __ldcs(src + c));
@@ -929,20 +1140,25 @@ __global__ void k_scatter_rows(const double* __restrict__ block, int64_t n_serie
 }
 
 cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, const int32_t* row, double* out, int ld,
-                            cudaStream_t st) {
+                            cudaStream_t st, const int64_t* count, const uint8_t* skip) {
     if (n_series <= 0 || n_cols <= 0) return cudaSuccess;
-    k_scatter_rows<<<grid_for(n_series * 32, 256), 256, 0, st>>>(block, n_series, n_cols, row, out, ld);
+    k_scatter_rows<<<grid_for(n_series * 32, 256), 256, 0, st>>>(block, n_series, n_cols, row, out, ld, count, skip);
     return cudaGetLastError();
 }
 
 // One warp per series, as k_check_views, but every series gets its own verdict instead of the call getting one
 __global__ void k_defer_check(const float* __restrict__ values, int64_t n_values, const int64_t* __restrict__ begin,
                               const int32_t* __restrict__ len, int64_t n_series, int32_t max_len, int64_t* __restrict__ vbegin,
-                              int32_t* __restrict__ vlen, uint8_t* __restrict__ reject, unsigned long long* first) {
+                              int32_t* __restrict__ vlen, uint8_t* __restrict__ reject, unsigned long long* first,
+                              int keep_unused) {
     const int lane = threadIdx.x & 31;
     int64_t w = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
     const int64_t n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (; w < n_series; w += n_warps) {                  // warp-uniform
+        if (keep_unused && reject[w] == DEFER_UNUSED) {
+            if (lane == 0) { vbegin[w] = 0; vlen[w] = 1; }
+            continue;
+        }
         int64_t b = w * (int64_t)max_len;
         int32_t l = max_len;
         int why = 0;
@@ -967,10 +1183,10 @@ __global__ void k_defer_check(const float* __restrict__ values, int64_t n_values
 
 cudaError_t defer_check(const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
                         int64_t n_series, int32_t max_len, int64_t* vbegin, int32_t* vlen, uint8_t* reject,
-                        unsigned long long* first, cudaStream_t st) {
+                        unsigned long long* first, cudaStream_t st, bool keep_unused) {
     if (n_series <= 0) return cudaSuccess;
     k_defer_check<<<grid_for(n_series * 32, 256), 256, 0, st>>>(d_values, n_values, d_begin, d_len, n_series, max_len,
-                                                                vbegin, vlen, reject, first);
+                                                                vbegin, vlen, reject, first, keep_unused ? 1 : 0);
     return cudaGetLastError();
 }
 

@@ -41,6 +41,7 @@ struct CsrWorkspace {
     size_t caps[16] = {0};
     CsrInfo* h_info = nullptr;    // pinned
     CsrInfo* d_info = nullptr;
+    bool frozen = false;          // reserve() fails instead of growing a buffer (a prepared, enqueue-only call)
     void release();
     cudaError_t reserve(int slot, size_t bytes);
     cudaError_t init_info();
@@ -130,6 +131,7 @@ struct StackedWorkspace {
     bool keys_f64 = false;        //   float64 ones
     void* bufs[32] = {nullptr};
     size_t caps[32] = {0};
+    bool frozen = false;          // reserve() fails instead of growing a buffer (a prepared, enqueue-only call)
     cudaError_t reserve(int slot, size_t bytes);
     cudaError_t keep_ids(const int64_t* d_src, int64_t n, cudaStream_t st);   // d_uid = a copy of n union ids
     void release();
@@ -166,12 +168,39 @@ int stacked_roll(StackedWorkspace& S, CsrWorkspace& W, int32_t rolling_direction
 // packages and n_union, copied to h_info (the caller synchronises).  bound >= the number of packages.
 int stacked_sub(StackedWorkspace& S, CsrWorkspace& W, int32_t L, int64_t bound, cudaStream_t st, std::string* msg);
 
+// Deferred stage (tsfx_extract_long_deferred): stacked_stage of n rows of which only [0, *n_live) count (n_live
+// nullptr: all n), enqueue-only.  The rows from *n_live on are made to sort after every live row, so the live rows
+// take the order, union rows and staged layout that stacked_stage gives them alone; the kind counting sort drops them
+// with the rows whose code is out of range (the bad_kind flag stays on the device, as nan_keys does).  The union size
+// goes to S.d_info->n_union, the union ids below max_ids to out_ids[0 .. n_union), the first id past them to *id_past.
+// Nothing is copied to the host, and S and W must hold what stacked_defer_reserve reserved for at least n rows.
+int stacked_stage_deferred(StackedWorkspace& S, CsrWorkspace& W, const int64_t* d_ids, const uint64_t* d_keys, int keys_f64,
+                           const float* d_values, const void* d_kinds, int kinds_i64, int n_kinds, int64_t n,
+                           const int64_t* d_n_live, int64_t max_ids, int64_t* out_ids, int64_t* id_past, cudaStream_t st,
+                           std::string* msg);
+
+// Every buffer stacked_stage_deferred of n rows and n_kinds kinds uses, with or without sort keys
+int stacked_defer_reserve(StackedWorkspace& S, CsrWorkspace& W, int64_t n, int n_kinds, std::string* msg);
+
+// After stacked_stage_deferred: kind k's series in the fixed slots [k * max_ids, (k + 1) * max_ids), in series order.  A
+// live series gets its view (sbegin, slen) and union row (srow); the other slots, and every slot of a call the stage
+// rejects (a kind code out of range, a NaN sort key, more than max_ids union rows), get reject reason DEFER_UNUSED.
+// live[k] = kind k's live series.
+cudaError_t stacked_slots(const StackedWorkspace& S, int n_kinds, int64_t max_ids, int64_t* sbegin, int32_t* slen,
+                          int32_t* srow, uint8_t* reject, int64_t* live, cudaStream_t st);
+
+// Last step of a deferred long call: *n_ids (0 for a rejected call), INT64_MAX in out_ids[*n_ids .. max_ids), and, if
+// the status words record this call (tsfx.h "Deferred input check"), its call-wide reasons and the id its report names.
+cudaError_t stacked_defer_report(const StackedWorkspace& S, int64_t max_ids, const int64_t* id_past, const int32_t* srow,
+                                 int64_t* out_ids, int64_t* n_ids, int64_t* status, cudaStream_t st);
+
 // out[r * ld + c] = NaN for r < n_rows, c < n_cols
 cudaError_t stacked_fill_nan(double* out, int64_t n_rows, int n_cols, int ld, cudaStream_t st);
 
-// out[row[s] * ld + c] = block[s * n_cols + c] for s < n_series, c < n_cols (one warp per row)
+// out[row[s] * ld + c] = block[s * n_cols + c] for s < n_series, c < n_cols (one warp per row).  count (device, may be
+// nullptr): only s < *count; skip (may be nullptr): not the series with skip[s] != 0.
 cudaError_t stacked_scatter(const double* block, int64_t n_series, int n_cols, const int32_t* row, double* out, int ld,
-                            cudaStream_t st);
+                            cudaStream_t st, const int64_t* count = nullptr, const uint8_t* skip = nullptr);
 
 // Checked pass over caller-supplied device views (TSFX_FLAG_CHECK_DEVICE_INPUT), one launch: the longest series into
 // d_info->max_len, the first view with len < 1, begin < 0 or begin + len > n_values into d_info->bad_view_rev, and a NaN
@@ -183,10 +212,11 @@ void csr_check_views(CsrWorkspace& W, const float* d_values, int64_t n_values, c
 // values + s * max_len, begin == nullptr; CSR: the caller's view) its reject reason into reject[s] (DEFER_VIEW, DEFER_LONG
 // or DEFER_NAN, 0: none) and, per reason r, n_series - s of the first rejected series into first[r - 1] (atomicMax,
 // zeroed by the caller).  CSR: the private view of every series into vbegin / vlen, (0, 1) for a rejected one.
-enum { DEFER_VIEW = 1, DEFER_LONG, DEFER_NAN };
+// keep_unused: a series whose reject[s] is already DEFER_UNUSED (stacked_slots) keeps it, unreported.
+enum { DEFER_VIEW = 1, DEFER_LONG, DEFER_NAN, DEFER_UNUSED };
 cudaError_t defer_check(const float* d_values, int64_t n_values, const int64_t* d_begin, const int32_t* d_len,
                         int64_t n_series, int32_t max_len, int64_t* vbegin, int32_t* vlen, uint8_t* reject,
-                        unsigned long long* first, cudaStream_t st);
+                        unsigned long long* first, cudaStream_t st, bool keep_unused = false);
 
 // After the groups of a deferred-check call: NaN in every column of every rejected series (out[s * ld + c], c < n_cols),
 // then the call's report into the caller's status words (tsfx.h TSFX_STATUS_*).

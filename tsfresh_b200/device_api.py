@@ -42,6 +42,13 @@ input row numbers that torch gathers from x.
 is extract_features_device prepared once for a batch shape: each call only enqueues work on torch's current stream, so
 it overlaps other work and can be captured in a CUDA graph.  Its input is checked on the device (TSFX_FLAG_DEFER_CHECK):
 rejected series come out as NaN rows and check() raises the error at a sync point the caller chooses.
+
+    ex = DeviceLongExtractor(max_rows, max_ids, max_length, kinds=[...])
+    X, row_ids, n_ids = ex(ids, values, sort, kind, n_rows=None, out=X)   # enqueues only
+    ex.check()
+
+is the same for extract_features_long_device: the rows are grouped on the device into a result of max_ids rows
+(tsfx_extract_long_deferred), the number of ids stays on the device, and the data errors wait for check().
 """
 import numbers
 
@@ -401,7 +408,143 @@ def extract_features_long_device(ids, values, sort=None, kind=None, *, kinds=Non
     return X, row_ids, columns
 
 
+class DeviceLongExtractor:
+    """extract_features_long_device prepared for one shape, for calls that only enqueue work.
+
+        ex = DeviceLongExtractor(max_rows, max_ids, max_length, kinds=[...])
+        X, row_ids, n_ids = ex(ids, values, sort=None, kind=None, n_rows=None, out=None)
+        ex.check()
+
+    A call takes at most max_rows long-format rows (ids, values, sort, kind as extract_features_long_device takes them,
+    rows in any order, times not offered) with at most max_ids distinct ids and (id, kind) series of at most max_length
+    samples.  kinds names the kind codes 0 .. K-1 (at most 64; None: one kind, "value"); default_fc_parameters and
+    kind_to_fc_parameters are as for extract_features_long_device, and `columns` are the names of ALL kinds' columns.
+    device: the CUDA device of the inputs (default: the current one).
+
+    The constructor compiles the plans, checks max_length against every plan's length limit (ValueError) and prepares a
+    private library context once: the stage's buffers for max_rows rows (about 90 bytes per row), the slot and check
+    buffers of K x max_ids series (29 bytes each), a staging block per kind (max_ids x its columns x 8 bytes) and what
+    DeviceExtractor prepares per plan for max_ids series of max_length samples.
+
+    A call checks the tensors' metadata at once (TypeError / ValueError, nothing enqueued): the layout checks of
+    extract_features_long_device, at most max_rows rows, one device, `out`, and n_rows.  It then only enqueues work on
+    torch's current stream: no host synchronisation, no allocation in the library, no read of device memory on the host.
+    values other than float32 are rounded to float32 on the device.  n_rows, a 0-d int64 CUDA tensor, makes only rows
+    [0, n_rows) count, so a captured graph can be replayed with another row count every step.
+
+    Returns X (float64 [max_ids, len(columns)]), row_ids (int64 [max_ids]) and n_ids (0-d int64), all on the device.
+    Rows [0, n_ids) of X are extract_features_long_device's rows for the same data, ids ascending in row_ids, and the
+    rows past n_ids are NaN, with row_ids 2**63 - 1, so row_ids stays ascending.  Unlike extract_features_long_device,
+    whose result has no columns for a kind without rows, X always has every kind's columns: a kind without rows in the
+    call has NaN columns.  With the longest series of every kind equal to max_length the rows are equal bit for bit; a
+    shorter longest series may select other kernel variants, which agree within the oracle parity.
+
+    The data are checked on the device.  A kind code outside 0 .. K-1, a NaN float64 sort key or more than max_ids
+    distinct ids reject the whole call (X all NaN, n_ids 0); a NaN value or more than max_length samples in the series
+    of an (id, kind) pair make that series' cells NaN in its kind's columns.  check() synchronises the device and raises
+    the ValueError of the first call since the last check() that met such an error, then forgets it: the message of
+    extract_features_long_device for a kind code, a NaN sort key or a NaN value; a message naming max_ids or max_length
+    and the id for the two limits.  impute_function and times (linear_trend_timewise) are not offered, as for
+    DeviceExtractor: imputation synchronises, and times would add a column only some calls could fill."""
+
+    def __init__(self, max_rows, max_ids, max_length, *, kinds=None, default_fc_parameters=None,
+                 kind_to_fc_parameters=None, device=None):
+        import torch
+        for name, v, top in (("max_rows", max_rows, _MAX_ROWS), ("max_ids", max_ids, _I32_MAX),
+                             ("max_length", max_length, _I32_MAX)):
+            if not isinstance(v, numbers.Integral) or not 1 <= v <= top:
+                raise ValueError("%s must be an integer in 1 .. %d, got %r" % (name, top, v))
+        self.max_rows, self.max_ids, self.max_length = int(max_rows), int(max_ids), int(max_length)
+        kinds = ["value"] if kinds is None else list(kinds)
+        if not 1 <= len(kinds) <= 64:
+            raise ValueError("between 1 and 64 kinds, %d named" % len(kinds))
+        if len(set(map(str, kinds))) != len(kinds):
+            raise ValueError("kinds must have distinct names: %r" % (kinds,))
+        _check_colname(*kinds)
+        self.kinds = kinds
+        self._plans, self.columns = _plans(kinds, default_fc_parameters, kind_to_fc_parameters)
+        for kind, plan in zip(kinds, self._plans):
+            limit = _lib.plan_max_len(plan)
+            if self.max_length > limit:
+                raise ValueError("series of %d samples exceed the limit of kind %r's settings (%d samples)"
+                                 % (self.max_length, kind, limit))
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        if self.device.type != "cuda":
+            raise ValueError("device must be a CUDA device, got %s" % self.device)
+        self._open()
+
+    def _open(self):
+        """The private context, its prepared shape and the status words (tsfx.h "Deferred long format")."""
+        import torch
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self._ctx = _lib.Context(self.device.index)
+        self._dps = [None if p.n_cols == 0 else _device_plan(self._ctx, p) for p in self._plans]
+        self._ctx.prepare_long(self._dps, self.max_rows, self.max_ids, self.max_length)
+        self._status = torch.zeros(_lib.STATUS_WORDS, dtype=torch.int64, device=self.device)
+        self._ctx.set_status(self._status.data_ptr())
+
+    def __call__(self, ids, values, sort=None, kind=None, n_rows=None, out=None):
+        import torch
+        n, _ = _long_layout(ids, values, sort, kind, self.kinds, None)
+        if n > self.max_rows:
+            raise ValueError("%d rows, the extractor was built for at most %d" % (n, self.max_rows))
+        if n_rows is not None:
+            if not isinstance(n_rows, torch.Tensor):
+                raise TypeError("n_rows must be a torch.Tensor, not %s" % type(n_rows).__name__)
+            if n_rows.dtype != torch.int64 or n_rows.ndim != 0:
+                raise ValueError("n_rows must be a 0-d int64 tensor, got %s of shape %s" % (n_rows.dtype, tuple(n_rows.shape)))
+        width = len(self.columns)
+        if out is not None:
+            _check_out(out, self.max_ids, width)
+        dev = self.device
+        for name, t in (("ids", ids), ("values", values), ("sort", sort), ("kind", kind), ("n_rows", n_rows), ("out", out)):
+            if t is not None and t.device != dev:
+                raise ValueError("%s is on %s, the extractor on %s" % (name, t.device, dev))
+        with torch.cuda.device(dev):
+            X = out if out is not None else torch.empty((self.max_ids, width), dtype=torch.float64, device=dev)
+            row_ids = torch.empty(self.max_ids, dtype=torch.int64, device=dev)
+            n_ids = torch.empty((), dtype=torch.int64, device=dev)
+            v = values.contiguous() if values.dtype == torch.float32 else values.to(torch.float32).contiguous()
+            i, s = ids.contiguous(), None if sort is None else sort.contiguous()
+            k = None if kind is None else kind.contiguous()
+            ctx = self._ctx
+            with ctx.lock:
+                # bound to the stream it last ran on, as DeviceExtractor: see there
+                ctx.set_stream(torch.cuda.current_stream(dev).cuda_stream or _lib.STREAM_LEGACY)
+                ctx.extract_long_deferred(i.data_ptr() if n else 0, 0 if s is None else s.data_ptr(),
+                                          s is not None and s.dtype == torch.float64, v.data_ptr() if n else 0,
+                                          0 if k is None else k.data_ptr(), k is not None and k.dtype == torch.int64, n,
+                                          0 if n_rows is None else n_rows.data_ptr(), row_ids.data_ptr(), n_ids.data_ptr(),
+                                          X.data_ptr() if width else 0, X.stride(0) if width else 0)
+        return X, row_ids, n_ids
+
+    def check(self):
+        """Synchronises the device; raises the ValueError of the first call since the last check() that met a data
+        error (then forgets it)."""
+        import torch
+        torch.cuda.synchronize(self.device)
+        st = self._status.cpu().tolist()
+        if st[_lib.STATUS_BAD] == 0:
+            return
+        self._status[_lib.STATUS_BAD] = 0
+        torch.cuda.synchronize(self.device)
+        what = "tsfx_stage_long_stacked"            # the eager call's messages name the stage that raises them
+        if st[_lib.STATUS_KIND]:
+            raise ValueError("%s: a kind code is outside 0 .. %d" % (what, len(self.kinds) - 1))
+        if st[_lib.STATUS_KEY_NAN]:
+            raise _lib.NanValuesError("%s: the float64 sort keys contain NaN" % what)
+        if st[_lib.STATUS_IDS]:
+            raise ValueError("%d distinct ids, more than max_ids=%d: id %d is the first past them"
+                             % (st[_lib.STATUS_IDS], self.max_ids, st[_lib.STATUS_ID]))
+        if st[_lib.STATUS_NAN] >= 0:
+            raise _lib.NanValuesError("%s: the value column contains NaN" % what)
+        raise ValueError("the series of id %d and kind %r is longer than max_length=%d"
+                         % (st[_lib.STATUS_ID], self.kinds[st[_lib.STATUS_LONG] // self.max_ids], self.max_length))
+
+
 _I32_MAX = (1 << 31) - 1
+_MAX_ROWS = (1 << 31) - 2 - 64 * 64
 
 
 def _roll_args(rolling_direction, max_timeshift, min_timeshift):
